@@ -76,8 +76,9 @@ struct TcCfg {
 };
 
 // kmask: bit (tap * 2 + half) = 0 skips the MMAs of that channel half of that tap (all-zero weights of a pixel-pair folded
-// conv, see net.cu fold_pixel_pairs; single-chunk layers only)
-template <int MODE, int CIN, int NT, int EB>
+// conv, see net.cu fold_pixel_pairs; single-chunk layers only).  GENERIC: outputs that are not NHWC at conv resolution with
+// whole channel tiles (NCHW maps, 1.1**x, upsampling); the other variant has only the NHWC epilogue (see wg_epilogue).
+template <int MODE, int CIN, int NT, int EB, bool GENERIC>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ S2Maps s2maps, const ConvParams p,
                const uint8_t* __restrict__ wpack, int tiles_x, int tiles_y, int num_tiles, int stages, unsigned kmask) {
@@ -205,7 +206,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
       }
       wgmma_wait<0>();
       if (wlane == 0) mbar_arrive(&empty[prev]);
-      wg_epilogue<NT>(p, acc, p.bias, n, y0, x0, blockIdx.y * NT, t);
+      wg_epilogue<NT, GENERIC ? kEpiGeneric : kEpiNhwc>(p, acc, p.bias, n, y0, x0, blockIdx.y * NT, t);
     }
   }
 }
@@ -305,11 +306,12 @@ bool tc_conv_supported(const ConvParams& p, int ksize, int stride) {
 
 template <int MODE, int CIN, int NT, int EB>
 static int launch_inst(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream, bool set_attr_only) {
-  auto kern = conv_tc_kernel<MODE, CIN, NT, EB>;
-  if (set_attr_only) {
-    B2R_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 /* plans of one instantiation differ in stages */));
+  if (set_attr_only) {   // plans of one instantiation differ in stages
+    B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     return B200ROMP_OK;
   }
+  auto kern = p.cout % NT == 0 && tc_nhwc_out(p, p.cout) ? conv_tc_kernel<MODE, CIN, NT, EB, false> : conv_tc_kernel<MODE, CIN, NT, EB, true>;
   CUtensorMap tm;
   memcpy(&tm, plan.tmap_in, sizeof(tm));
   S2Maps s2;

@@ -230,23 +230,108 @@ __device__ __forceinline__ void wg_store2(const ConvParams& p, int n, int oy, in
   }
 }
 
+// output NHWC at conv resolution, channels [.., co_end) inside the op's channels: no NCHW maps, 1.1**x or upsampling
+__host__ __device__ __forceinline__ bool tc_nhwc_out(const ConvParams& p, int co_end) {
+  return p.up == 1 && !p.out_nchw && p.pow_channel < 0 && co_end <= p.cout;
+}
+
+__device__ __forceinline__ float2 res_pair(uint32_t r) {
+  const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&r);
+  return make_float2(__low2float(v), __high2float(v));
+}
+__device__ __forceinline__ float2 res_pair(float2 r) { return r; }
+
+// NHWC output at conv resolution, whole channel tile.  A thread's fragments lie on 4 pixel rows; the residual pairs of ROWS
+// of them are loaded into registers before the first store of those rows.  `out` and `res` are plain pointers that the
+// compiler must assume to alias, so loads interleaved with stores would wait for one memory round trip per fragment (16
+// per tile at NT = 32, 32 at NT = 64); this way a tile pays 4 / ROWS.  ROWS keeps the staged residual at 16 registers.  Nets never give an op's output the buffer of its
+// residual (net.cu buffer planner), so the reordering cannot change a result.
+template <int NT, typename RT, int ROWS = (NT / 8) * (int)sizeof(RT) <= 16 ? 4 : (NT / 8) * (int)sizeof(RT) <= 32 ? 2 : 1>
+__device__ __forceinline__ void wg_epilogue_nhwc(const ConvParams& p, const float (&acc)[2][NT / 2], int n, int y0, int x0, int co0,
+                                                 int w, int l, bool linear) {
+  // row m = 64h + 16w + l/4 + 8e of the tile is pixel pix0 + (8h + e) * dpix of the frame: the thread's fragments sit at 4
+  // pixel rows, and channel group j is a constant byte offset from them
+  const int dpix = linear ? 8 : p.Wout;
+  auto pix0 = [&](int frame) -> size_t {
+    return linear ? ((size_t)frame * p.Hout + y0) * p.Wout + x0 + 16 * w + (l >> 2)
+                  : ((size_t)frame * p.Hout + y0 + 2 * w) * p.Wout + x0 + (l >> 2);
+  };
+  const int c = co0 + 2 * (l & 3);
+  const uint8_t* rbase = nullptr;
+  int rstep = 0;
+  if (p.res != nullptr) {
+    rbase = reinterpret_cast<const uint8_t*>(p.res) + (pix0(p.res_broadcast ? 0 : n) * p.res_C + p.res_c_off + c) * (sizeof(RT) / 2);
+    rstep = dpix * p.res_C * (int)(sizeof(RT) / 2);
+  }
+  const int ob = p.out_dtype == B200ROMP_BF16 ? 2 : 4;
+  uint8_t* obase = reinterpret_cast<uint8_t*>(p.out) + (pix0(n) * p.out_C + p.out_c_off + c) * ob;
+  const int ostep = dpix * p.out_C * ob;
+#pragma unroll
+  for (int q0 = 0; q0 < 4; q0 += ROWS) {   // fragment row q = 2h + e
+    RT rv[ROWS][NT / 8];
+    if (p.res != nullptr) {
+#pragma unroll
+      for (int qq = 0; qq < ROWS; ++qq) {
+        const int q = q0 + qq;
+        const RT* r = reinterpret_cast<const RT*>(rbase + (8 * (q >> 1) + (q & 1)) * rstep);
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) rv[qq][j] = r[4 * j];   // channel 8j: RT holds 2 channels
+      }
+    }
+#pragma unroll
+    for (int qq = 0; qq < ROWS; ++qq) {
+      const int q = q0 + qq, h = q >> 1, e = q & 1;
+      uint8_t* o = obase + (8 * h + e) * ostep;
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        float a = acc[h][4 * j + 2 * e], b = acc[h][4 * j + 2 * e + 1];   // bias included
+        if (p.res != nullptr) { const float2 r = res_pair(rv[qq][j]); a += r.x; b += r.y; }
+        if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+        if (ob == 2) reinterpret_cast<__nv_bfloat162*>(o)[4 * j] = __floats2bfloat162_rn(a, b);
+        else reinterpret_cast<float2*>(o)[4 * j] = make_float2(a, b);
+      }
+    }
+  }
+}
+
 // Epilogue of one 128-pixel x NT-channel tile held as two m64 accumulators (rows 0-63 / 64-127) by a warpgroup: row m of the
 // tile is pixel (m / 8, m % 8) of the 16 x 8 tile at (y0, x0) of frame n (linear: pixel (y0, x0 + m), a 128-wide row).  wgmma fragment: thread (warp w, lane l) holds,
 // for each 8-column group j, columns 8j + 2(l%4) + {0,1} of rows 16w + l/4 (regs 4j, 4j+1) and 16w + l/4 + 8 (4j+2, 4j+3).
-template <int NT>
-__device__ __forceinline__ void wg_epilogue(const ConvParams& p, const float (&acc)[2][NT / 2], const float* __restrict__ bias, int n,
+// The accumulators are consumed: the bias is added in place.  PATH selects the code compiled in: kEpiNhwc when the caller
+// guarantees an NHWC conv-resolution output (tc_nhwc_out), kEpiGeneric when it guarantees the opposite, kEpiAny decides per
+// tile.  A kernel that carries both needs about 40 registers more than one with kEpiNhwc alone.
+constexpr int kEpiNhwc = 0, kEpiGeneric = 1, kEpiAny = 2;
+template <int NT, int PATH = kEpiAny>
+__device__ __forceinline__ void wg_epilogue(const ConvParams& p, float (&acc)[2][NT / 2], const float* __restrict__ bias, int n,
                                             int y0, int x0, int co0, int wg_thread, bool linear = false) {
   const int w = wg_thread >> 5, l = wg_thread & 31;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
+  if (PATH == kEpiNhwc || (PATH == kEpiAny && tc_nhwc_out(p, co0 + NT))) {
 #pragma unroll
     for (int j = 0; j < NT / 8; ++j) {
       const int c = co0 + 8 * j + 2 * (l & 3);
       const float b0 = __ldg(bias + c), b1 = __ldg(bias + c + 1);
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int m = 64 * h + 16 * w + (l >> 2) + 8 * e;
-        wg_store2(p, n, linear ? y0 : y0 + (m >> 3), linear ? x0 + m : x0 + (m & 7), c, acc[h][4 * j + 2 * e] + b0, acc[h][4 * j + 2 * e + 1] + b1);
+      for (int h = 0; h < 2; ++h) {
+        acc[h][4 * j] += b0; acc[h][4 * j + 1] += b1; acc[h][4 * j + 2] += b0; acc[h][4 * j + 3] += b1;
+      }
+    }
+    if (p.res != nullptr && p.res_dtype == B200ROMP_F32) wg_epilogue_nhwc<NT, float2>(p, acc, n, y0, x0, co0, w, l, linear);
+    else wg_epilogue_nhwc<NT, uint32_t>(p, acc, n, y0, x0, co0, w, l, linear);
+    return;
+  }
+  if constexpr (PATH != kEpiNhwc) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int c = co0 + 8 * j + 2 * (l & 3);
+        const float b0 = __ldg(bias + c), b1 = __ldg(bias + c + 1);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 64 * h + 16 * w + (l >> 2) + 8 * e;
+          wg_store2(p, n, linear ? y0 : y0 + (m >> 3), linear ? x0 + m : x0 + (m & 7), c, acc[h][4 * j + 2 * e] + b0,
+                    acc[h][4 * j + 2 * e + 1] + b1);
+        }
       }
     }
   }

@@ -3,7 +3,10 @@
     python tools/op_profile.py [--batch 64] [--iters 5] > op_profile.md
 
 Ops are launched one by one (no CUDA graph) with a CUDA event between them, so the numbers are warm-cache device
-times in network order; FLOP counts are algorithmic (2*MAC of the conv at its own resolution)."""
+times in network order; FLOP counts are algorithmic (2*MAC of the conv at its own resolution).  Bytes are algorithmic too:
+the input channel slice, the output and the residual read once each, at the activation size of the precision (2 bytes in
+bf16, 4 otherwise; the few fp32 tensors of a bf16 net are counted at 2).  Low-intensity layers are bounded by these bytes,
+not by FLOPs, so GB/s is the rate to set against the HBM bandwidth."""
 import argparse
 import os
 import re
@@ -27,6 +30,7 @@ def main():
     B = args.batch
     nb, io = graph.build_romp(synth.romp_state_dict(0), 0, args.precision, _lib.U8, max_batch=B)
     lib = nb.lib
+    eb = 2 if args.precision == "bf16" else 4
     frames = torch.randint(0, 256, (B, 512, 512, 3), dtype=torch.uint8, device="cuda")
     ext = {}
     if io is not None:
@@ -40,36 +44,39 @@ def main():
     rows = []
     for l, t in zip(lines, us):
         if " sum " in l:
-            rows.append((t, 0.0, l))
+            rows.append((t, 0.0, 0.0, l))
             continue
         m = re.search(r"k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x(\d+)x\d+\]", l)
         k, s, cin, cout, H, W = (int(x) for x in m.groups())
         k2 = 3 if k == 13 else k * k
         ho, wo = H // s, W // s
+        up = int(re.search(r"up(\d)", l).group(1))
         flop = 2.0 * B * ho * wo * cin * cout * k2
-        rows.append((t, flop, l))
+        nbytes = eb * B * (H * W * cin + ho * wo * up * up * cout * (2 if "res t-1" not in l else 1))
+        rows.append((t, flop, nbytes, l))
     total = sum(r[0] for r in rows)
     tf = sum(r[1] for r in rows)
-    print(f"# per-op profile, batch {B}: {len(rows)} ops, {total / 1000:.3f} ms, {tf / total / 1e6:.1f} TFLOP/s overall\n")
+    tb = sum(r[2] for r in rows)
+    print(f"# per-op profile, batch {B}: {len(rows)} ops, {total / 1000:.3f} ms, {tf / total / 1e6:.1f} TFLOP/s, {tb / total / 1e3:.0f} GB/s overall\n")
     # by class
     cls = {}
-    for t, f, l in rows:
+    for t, f, nb_, l in rows:
         if " sum " in l:
             ms = re.search(r"out t\d+\[(\d+)x\d+x(\d+)\]", l)
-            a = cls.setdefault(f"sum @{ms.group(1)} c{ms.group(2)} terms{l.count('up')}", [0, 0.0, 0.0])
+            a = cls.setdefault(f"sum @{ms.group(1)} c{ms.group(2)} terms{l.count('up')}", [0, 0.0, 0.0, 0.0])
             a[0] += 1; a[1] += t
             continue
         m = re.search(r"(wgmma|simt) +k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x", l)
         key = f"{m.group(1)} k{m.group(2)} s{m.group(3)} {m.group(4)}->{m.group(5)} @{m.group(6)}" + (" epi" + l.split("epi")[1][0] if "epi" in l else "") + \
-              (" up" + re.search(r"up(\d)", l).group(1))
-        a = cls.setdefault(key, [0, 0.0, 0.0])
-        a[0] += 1; a[1] += t; a[2] += f
-    print("| class | ops | total us | share | avg us | TFLOP/s |\n|---|---:|---:|---:|---:|---:|")
-    for k, (n, t, f) in sorted(cls.items(), key=lambda kv: -kv[1][1]):
-        print(f"| {k} | {n} | {t:.1f} | {100 * t / total:.1f}% | {t / n:.1f} | {f / t / 1e6:.0f} |")
-    print("\n| us | TFLOP/s | op |\n|---:|---:|---|")
-    for t, f, l in sorted(rows, key=lambda r: -r[0])[:args.top]:
-        print(f"| {t:.1f} | {f / t / 1e6:.0f} | `{l.strip()}` |")
+              (" up" + re.search(r"up(\d)", l).group(1)) + (" res" if "res t-1" not in l else "")
+        a = cls.setdefault(key, [0, 0.0, 0.0, 0.0])
+        a[0] += 1; a[1] += t; a[2] += f; a[3] += nb_
+    print("| class | ops | total us | share | avg us | TFLOP/s | GB/s |\n|---|---:|---:|---:|---:|---:|---:|")
+    for k, (n, t, f, nb_) in sorted(cls.items(), key=lambda kv: -kv[1][1]):
+        print(f"| {k} | {n} | {t:.1f} | {100 * t / total:.1f}% | {t / n:.1f} | {f / t / 1e6:.0f} | {nb_ / t / 1e3:.0f} |")
+    print("\n| us | TFLOP/s | GB/s | op |\n|---:|---:|---:|---|")
+    for t, f, nb_, l in sorted(rows, key=lambda r: -r[0])[:args.top]:
+        print(f"| {t:.1f} | {f / t / 1e6:.0f} | {nb_ / t / 1e3:.0f} | `{l.strip()}` |")
 
 
 if __name__ == "__main__":
