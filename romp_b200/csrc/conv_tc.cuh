@@ -14,7 +14,8 @@ struct S2Maps {
 };
 
 struct TcConvPlan {
-  int kind = 0;                 // kernel family: 10 = 1x1, 30 = 3x3, 32 = 3x3 stride 2, 33 = u8 stem, 13 = conv1d; 0 = none
+  int kind = 0;                 // kernel family: 10 = 1x1, 30 = 3x3, 32 = 3x3 stride 2, 33 = u8 stem, 13 = conv1d,
+                                // 60 = fused 3x3 BasicBlock (conv_block_tc.cu); 0 = none
   int cin = 0, cout = 0, nt = 0;  // channels, output channels per CTA
   int eb = 2;                   // operand element bytes: 2 = bf16, 4 = fp32 storage consumed as TF32
   int grid_x = 0, grid_y = 0, stages = 0;
@@ -27,6 +28,9 @@ struct TcConvPlan {
   unsigned kmask = 0xFFFFFFFFu;
   const void* encoded_in = nullptr;   // conv1d engine: input pointer / batch the tensor map was encoded for (external inputs)
   int encoded_batch = 0;
+  void* d_wpack2 = nullptr;           // fused block: conv2's weight image (d_wpack holds conv1's)
+  const float* d_bias1 = nullptr;     // fused block: conv1's bias [64] (conv2's is ConvParams::bias)
+  int fold = 0;                       // fused block: runs on the pixel-pair view (both convs folded)
   std::string describe() const;
 };
 
@@ -45,5 +49,12 @@ bool tc_stem_supported(const ConvParams& p, int ksize, int stride);
 int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, bool out_final, TcConvPlan* plan,
                     std::vector<void*>* allocs);
 int tc_stem_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
+// fused BasicBlock engine (conv_block_tc.cu): y = relu(conv2(relu(conv1(x) + b1)) + b2 + x), 3x3 stride 1, 64 -> 64 -> 64
+// bf16 NHWC.  `p` describes the block as one op: input and residual x (the same channel slice), output y, bias b2; when
+// `fold` the weights are already the pixel-pair folded ones and `p` the pixel-pair view.
+bool tc_block_supported(const ConvParams& p);
+int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, bool fold, int sm_count,
+                     TcConvPlan* plan, std::vector<void*>* allocs);
+int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
 
 }  // namespace b200romp

@@ -49,6 +49,11 @@ struct Op {
   TcConvPlan tc;                       // tensor-core plan (packed weights, tensor maps)
   int lane = 0;                        // concurrency lane inside the captured CUDA graph (b200romp_net_set_lane)
   int fold = 0;                        // 1 = runs as a pixel-pair folded 64->64 conv on the [H, W/2, 64] view (fold_pixel_pairs)
+  // fused BasicBlock (fuse_basic_blocks): d describes the block (in and res = x, out = y, bias = b2), w_host / b_host are
+  // conv1's, w2_host / b2_host conv2's, `mid` is the intermediate tensor that no longer gets a buffer
+  int block = 0;
+  int mid = -1;
+  std::vector<float> w2_host, b2_host;
 };
 
 }  // namespace b200romp
@@ -303,6 +308,7 @@ static int enqueue_op(b200romp_net* net, Op& op, int batch, cudaStream_t stream)
   ConvParams p;
   int rc = fill_params(net, op, batch, &p);
   if (rc) return rc;
+  if (op.block) return tc_block_launch(op.tc, p, stream);
   if (op.d.ksize == 7) return launch_conv_generic(p, 7, op.d.stride, stream);
   if (op.d.ksize == 42) return launch_deconv4x4s2(p, stream);
   if (op.engine == B200ROMP_ENGINE_TCGEN05) return op.tc.kind == 13 ? tc_conv1d_launch(op.tc, p, stream) : tc_conv_launch(op.tc, p, stream);
@@ -377,9 +383,104 @@ static void fold_pixel_pairs(const std::vector<float>& w, const std::vector<floa
   *kmask = m;
 }
 
+// HRNet BasicBlocks relu(conv2(relu(conv1(x))) + x) whose convs are 3x3 stride-1 64->64 (or pixel-pair foldable 32->32) bf16
+// layers become one op on the fused block kernel (conv_block_tc.cu): the intermediate never reaches HBM and x is read once.
+// Ops i, i+1 fuse when conv2 reads exactly conv1's output, that tensor is internal and read by nothing else, and conv2's
+// residual is conv1's input slice.  A caller that binds the intermediate as an external tensor keeps the two convs.
+static bool is_bf16_block_conv(const b200romp_net* net, const Op& op) {
+  const b200romp_conv_desc& d = op.d;
+  const Tensor& ti = net->tensors[d.in];
+  const Tensor& to = net->tensors[d.out];
+  return op.kind == 0 && d.ksize == 3 && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
+         (d.engine == B200ROMP_ENGINE_AUTO || d.engine == B200ROMP_ENGINE_TCGEN05) && ti.dtype == B200ROMP_BF16 &&
+         to.dtype == B200ROMP_BF16 && !to.nchw && d.cin == d.cout && (d.cin == 64 || d.cin == 32);
+}
+
+static void fuse_basic_blocks(b200romp_net* net) {
+  const int nT = (int)net->tensors.size();
+  std::vector<int> reads(nT, 0), writes(nT, 0);
+  for (const Op& op : net->ops) {
+    ++reads[op.d.in];
+    ++writes[op.d.out];
+    if (op.kind == 1)
+      for (int k = 0; k < op.sum.n_terms; ++k) ++reads[op.sum.term[k]];
+    else if (op.d.res >= 0) ++reads[op.d.res];
+  }
+  std::vector<Op> fused;
+  fused.reserve(net->ops.size());
+  for (size_t i = 0; i < net->ops.size(); ++i) {
+    Op& a = net->ops[i];
+    if (i + 1 < net->ops.size()) {
+      Op& b = net->ops[i + 1];
+      const int x = a.d.in, t = a.d.out;
+      const Tensor& tx = net->tensors[x];
+      const Tensor& tt = net->tensors[t];
+      const int C = a.d.cin;
+      bool ok = is_bf16_block_conv(net, a) && is_bf16_block_conv(net, b) && a.d.res < 0 && b.d.cin == C && a.lane == b.lane &&
+                b.d.in == t && b.d.in_c_off == 0 && a.d.out_c_off == 0 && tt.C == C && !tt.external && !tt.constant &&
+                reads[t] == 1 && writes[t] == 1 && b.d.res == x && b.d.res_c_off == a.d.in_c_off && !b.d.res_broadcast &&
+                !tx.external && tx.H % 16 == 0;
+      bool fold = false;
+      if (ok && C == 32) {
+        fold = fold_eligible(net, a) && fold_eligible(net, b);   // the 32-channel kernel is the folded 64-channel one
+        ok = fold;
+      }
+      if (ok && C == 64) {
+        const Tensor& ty = net->tensors[b.d.out];
+        ok = !ty.external && tx.W % 8 == 0 && tx.C % 8 == 0 && a.d.in_c_off % 8 == 0 && ty.C % 8 == 0 && b.d.out_c_off % 8 == 0;
+      }
+      if (ok) {
+        Op f;
+        f.d = a.d;
+        f.d.out = b.d.out;
+        f.d.out_c_off = b.d.out_c_off;
+        f.d.res = x;
+        f.d.res_c_off = b.d.res_c_off;
+        f.block = 1;
+        f.fold = fold ? 1 : 0;
+        f.mid = t;
+        f.lane = a.lane;
+        f.w_host = std::move(a.w_host);
+        f.b_host = std::move(a.b_host);
+        f.w2_host = std::move(b.w_host);
+        f.b2_host = std::move(b.b_host);
+        fused.push_back(std::move(f));
+        ++i;
+        continue;
+      }
+    }
+    fused.push_back(std::move(a));
+  }
+  net->ops = std::move(fused);
+}
+
+// weights, biases and plan of a fused block op (the engine resolution of fuse_basic_blocks' ops)
+static int prepare_block(b200romp_net* net, Op& op, int max_batch) {
+  std::vector<float> w1 = op.w_host, b1 = op.b_host, w2 = op.w2_host, b2 = op.b2_host;
+  if (op.fold) {
+    unsigned kmask = 0;
+    fold_pixel_pairs(op.w_host, op.b_host, &w1, &b1, &kmask);
+    fold_pixel_pairs(op.w2_host, op.b2_host, &w2, &b2, &kmask);
+  }
+  op.coutPad = 64;
+  B2R_CUDA_OK(cudaMalloc(&op.d_bias, 64 * sizeof(float)));
+  net->device_allocs.push_back(op.d_bias);
+  B2R_CUDA_OK(cudaMemcpy(op.d_bias, b2.data(), 64 * sizeof(float), cudaMemcpyHostToDevice));
+  ConvParams p;
+  int rc = fill_params(net, op, max_batch, &p);
+  if (rc) return rc;
+  rc = tc_block_prepare(p, w1.data(), b1.data(), w2.data(), op.fold != 0, net->sm_count, &op.tc, &net->device_allocs);
+  if (rc) return rc;
+  op.engine = B200ROMP_ENGINE_TCGEN05;
+  op.w_host.clear(); op.w_host.shrink_to_fit();
+  op.w2_host.clear(); op.w2_host.shrink_to_fit();
+  return B200ROMP_OK;
+}
+
 int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   B2R_REQUIRE(net && !net->finalized && max_batch > 0, "finalize: bad arguments");
   B2R_CUDA_OK(cudaSetDevice(net->device));
+  fuse_basic_blocks(net);   // before liveness: a fused block's intermediate gets no buffer
   const int nT = (int)net->tensors.size(), nO = (int)net->ops.size();
   // ---- liveness over the linear op order
   for (int i = 0; i < nO; ++i) {
@@ -445,6 +546,11 @@ int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   for (int i = 0; i < nO; ++i) {
     Op& op = net->ops[i];
     if (op.kind == 1 || op.kind == 2) continue;
+    if (op.block) {
+      int rc = prepare_block(net, op, max_batch);
+      if (rc) return rc;
+      continue;
+    }
     int rc = upload_simt_weights(net, op);
     if (rc) return rc;
     op.engine = B200ROMP_ENGINE_SIMT;
@@ -684,7 +790,7 @@ int b200romp_net_read_tensor(b200romp_net* net, int tensor, int batch, void* dst
 int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
   if (!net || !buf || len <= 0) return B200ROMP_EINVAL;
   std::string s;
-  char line[256];
+  char line[384];
   for (size_t i = 0; i < net->ops.size(); ++i) {
     const Op& op = net->ops[i];
     const b200romp_conv_desc& d = op.d;
@@ -699,6 +805,16 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
       int n = snprintf(line, sizeof(line), "op%03zu sum     out t%d[%dx%dx%d] = relu%d( t%d", i, op.sum.out, to.H, to.W, to.C, op.sum.relu, op.sum.base);
       for (int k = 0; k < op.sum.n_terms; ++k) n += snprintf(line + n, sizeof(line) - n, " + up%d(t%d)", op.sum.up[k], op.sum.term[k]);
       snprintf(line + n, sizeof(line) - n, " )\n");
+      s += line;
+      continue;
+    }
+    if (op.block) {   // one launch, two convs: a folded block runs both of them on pixel pairs
+      const Tensor& tm = net->tensors[op.mid];
+      snprintf(line, sizeof(line),
+               "op%03zu wgmma   block k3 s1 %d->%d->%d in t%d[%dx%dx%d]+%d mid t%d[%dx%dx%d] out t%d[%dx%dx%d]+%d res t%d+%d up1 relu1 "
+               "bias1 bias2 [tc-block grid %d smem %d%s]\n",
+               i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
+               d.out_c_off, d.res, d.res_c_off, op.tc.grid_x, op.tc.smem_bytes, op.fold ? " conv1 pixel-pairs conv2 pixel-pairs" : "");
       s += line;
       continue;
     }

@@ -6,7 +6,9 @@ Ops are launched one by one (no CUDA graph) with a CUDA event between them, so t
 times in network order; FLOP counts are algorithmic (2*MAC of the conv at its own resolution).  Bytes are algorithmic too:
 the input channel slice, the output and the residual read once each, at the activation size of the precision (2 bytes in
 bf16, 4 otherwise; the few fp32 tensors of a bf16 net are counted at 2).  Low-intensity layers are bounded by these bytes,
-not by FLOPs, so GB/s is the rate to set against the HBM bandwidth."""
+not by FLOPs, so GB/s is the rate to set against the HBM bandwidth.  A fused BasicBlock op (`block k3`, conv_block_tc.cu)
+counts the FLOPs of both convs and moves its input once and its output once: the intermediate stays in shared memory and
+the residual is the block's own input, read from the staged input tile, so neither adds bytes."""
 import argparse
 import os
 import re
@@ -46,6 +48,11 @@ def main():
         if " sum " in l:
             rows.append((t, 0.0, 0.0, l))
             continue
+        mb = re.search(r"block k3 s1 (\d+)->(\d+)->(\d+) in t\d+\[(\d+)x(\d+)x\d+\]", l)
+        if mb:
+            c0, c1, c2, H, W = (int(x) for x in mb.groups())
+            rows.append((t, 2.0 * B * H * W * 9 * (c0 * c1 + c1 * c2), eb * B * H * W * (c0 + c2), l))
+            continue
         m = re.search(r"k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x(\d+)x\d+\]", l)
         k, s, cin, cout, H, W = (int(x) for x in m.groups())
         k2 = 3 if k == 13 else k * k
@@ -65,6 +72,11 @@ def main():
             ms = re.search(r"out t\d+\[(\d+)x\d+x(\d+)\]", l)
             a = cls.setdefault(f"sum @{ms.group(1)} c{ms.group(2)} terms{l.count('up')}", [0, 0.0, 0.0, 0.0])
             a[0] += 1; a[1] += t
+            continue
+        mb = re.search(r"block k3 s1 (\d+->\d+->\d+) in t\d+\[(\d+)x", l)
+        if mb:
+            a = cls.setdefault(f"wgmma block k3 {mb.group(1)} @{mb.group(2)} res", [0, 0.0, 0.0, 0.0])
+            a[0] += 1; a[1] += t; a[2] += f; a[3] += nb_
             continue
         m = re.search(r"(wgmma|simt) +k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x", l)
         key = f"{m.group(1)} k{m.group(2)} s{m.group(3)} {m.group(4)}->{m.group(5)} @{m.group(6)}" + (" epi" + l.split("epi")[1][0] if "epi" in l else "") + \
