@@ -38,23 +38,24 @@ def conv2d(x_nhwc, w, b=None, *, stride=1, relu=False, res=None, up=1, out_dtype
     return out
 
 
-def conv_ref(x_nhwc_f32, w, b=None, *, stride=1, relu=False, res=None, up=1, input_norm=0, pow_channel=-1):
-    """fp32 torch CPU reference of the fused op; returns NHWC."""
+def conv_ref(x_nhwc, w, b=None, *, stride=1, relu=False, res=None, up=1, input_norm=0, pow_channel=-1, device="cpu",
+             dtype=torch.float32):
+    """torch reference of the fused op, computed in `dtype` on `device` (default: fp32 on the CPU); returns NHWC.
+    w, b: numpy arrays or tensors; a residual with one frame is broadcast over the batch."""
     import torch.nn.functional as F
-    x = x_nhwc_f32.float().cpu().permute(0, 3, 1, 2)
+    x = x_nhwc.to(device=device, dtype=dtype).permute(0, 3, 1, 2)
     if input_norm:
         x = (x / 255.0) * 2.0 - 1.0
-    wt = torch.from_numpy(np.asarray(w, np.float32))
+    wt = torch.as_tensor(w).to(device=device, dtype=dtype)
+    bt = None if b is None else torch.as_tensor(b).to(device=device, dtype=dtype)
     if wt.ndim == 3:                                  # Conv1d along W
-        wt = wt[:, :, None, :]
-        y = F.conv2d(x, wt, None if b is None else torch.from_numpy(np.asarray(b, np.float32)), stride=1, padding=(0, 1))
+        y = F.conv2d(x, wt[:, :, None, :], bt, stride=1, padding=(0, 1))
     else:
-        y = F.conv2d(x, wt, None if b is None else torch.from_numpy(np.asarray(b, np.float32)), stride=stride,
-                     padding=w.shape[-1] // 2)
+        y = F.conv2d(x, wt, bt, stride=stride, padding=wt.shape[-1] // 2)
     if up > 1:
         y = F.interpolate(y, scale_factor=up, mode="nearest")
     if res is not None:
-        y = y + res.float().cpu().permute(0, 3, 1, 2)
+        y = y + res.to(device=device, dtype=dtype).permute(0, 3, 1, 2)
     if relu:
         y = F.relu(y)
     if pow_channel >= 0:
@@ -63,6 +64,6 @@ def conv_ref(x_nhwc_f32, w, b=None, *, stride=1, relu=False, res=None, up=1, inp
 
 
 def round_tf32(t):
-    """fp32 -> TF32 (10 mantissa bits, ties away from zero) like cvt.rna.tf32.f32; stays in fp32 containers."""
-    i = t.detach().cpu().float().contiguous().view(torch.int32)
+    """fp32 -> TF32 (10 mantissa bits, ties away from zero) like cvt.rna.tf32.f32; stays in fp32 containers on t's device."""
+    i = t.detach().float().contiguous().view(torch.int32)
     return ((i + 0x1000) & ~0x1FFF).view(torch.float32)

@@ -4,7 +4,7 @@ Each case builds the same block twice with NetBuilder: once as it is (the graph 
 the intermediate tensor, which keeps the two convs apart on the per-conv wgmma path.  The fused block keeps the K order of
 the per-conv kernel, so the two outputs must be bit-equal.  A comparison with the fp32 torch reference catches border bugs
 both paths might share.  Frames of 64x128 make tiles touch every border; batch 5 makes the persistent CTAs loop over tiles,
-batch 1 launches fewer tiles than SMs."""
+batch 1 launches fewer tiles than SMs, and the folded block at batch 9 gives some CTAs a third tile."""
 import numpy as np
 import pytest
 import torch
@@ -22,6 +22,7 @@ CASES = [
     ("c64_slice_64_of_192", 64, 5, 192, 64),
     ("c64_batch1", 64, 1, 64, 0),
     ("c32_pixel_pairs_batch1", 32, 1, 32, 0),
+    ("c32_pixel_pairs_batch9", 32, 9, 32, 0),      # 288 folded tiles on 132 CTAs: a third tile (and parity wrap) per CTA
 ]
 H, W = 64, 128
 
