@@ -10,7 +10,8 @@
  * input/output buffers; the library owns only packed constants and the conv-graph workspace.
  *
  * Device selection: entry points that take a handle (net, smpl, bev, tracks) make the handle's device current themselves;
- * the handle-less ones (parse, project, preprocess_bgr, pack_rows, bev_bv_input / parse3d / post, gather_rows) launch on
+ * the handle-less ones (parse, project, preprocess_bgr, pack_rows, bev_bv_input / parse3d / post / crop_post / long_merge,
+ * gather_rows) launch on
  * the CURRENT device - the caller must have made the device that owns the stream and the buffers current.
  *
  * Return convention: 0 = OK, negative = error (b200romp_last_error() gives the text).  "Nobody
@@ -229,6 +230,32 @@ int b200romp_bev_post(const float* betas, const float* verts_smil, const float* 
                       const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
                       const int* d_count, const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side,
                       float* pj2d_org, int* keep, int* sel, int* d_count_out, b200romp_stream stream);
+/* Long-image (crowd) mode, per-crop stage (bev/main.py:196-249, bev/split2process.py:41-58) for one chunk of crop frames
+ * (batch frames = crops crop0 .. crop0+batch-1 of the image, rows grouped by frame like bev_parse3d leaves them).  After
+ * SMPL-A / SMIL: merge babies, then per crop: drop the persons in the overlap with the neighbouring crops (cam x against
+ * crop_table[c][0] / [1]), project to crop pixels, suppressing_redundant_prediction_via_projection(conf_based=True),
+ * remove_outlier(scale_thresh=1), convert cam to the full image (cam *= [4]; cam[:,2] += [5], fp32).  The survivors are
+ * APPENDED in order to the acc_* rows (verts [6890,3], joints [71,3], thetas 72, betas 11, params_pred 146 with the crop's
+ * cam, conf 1, full-image cam 3) at the device-side running count acc_count[0] (at most acc_capacity rows);
+ * acc_count[1] counts every person detected in the crops so far (zero both before the first chunk of an image).
+ * crop_table: DEVICE fp32 [n_crops][6] = {left drop above, right drop below, projection size max(ch,cw),
+ * suppression threshold in pixels, cam scale, cam x shift}.  pj2d [cap,71,2], keep/sel [cap], cam_full [cap,3],
+ * acc_ctl [2] are scratch. */
+int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                           const float* thetas, const float* params_pred, const float* conf, const float* cam, const float* cam_trans,
+                           const long long* batch_ids, int batch, int capacity, const int* d_count, const float* crop_table,
+                           int crop0, float rel_scale_thresh, float* pj2d, int* keep, int* sel, float* cam_full, int acc_capacity,
+                           int* acc_count, int* acc_ctl, float* acc_verts, float* acc_joints, float* acc_thetas, float* acc_betas,
+                           float* acc_params_pred, float* acc_conf, float* acc_cam, b200romp_stream stream);
+/* Long-image mode, merged stage (bev/main.py:253-256) over the *d_count accumulated persons of one image (any number up
+ * to capacity, not bounded by 64): cam_trans from the full-image cam, projection with the full image's pad info
+ * offsets6 (HOST, [top,bottom,left,right,h,w]), conf-based suppression with nms_thresh * img_max_side / 640 (every pair below
+ * it at once), remove_outlier(scale_thresh=0.5).  removed [cap] flags; sel [cap] = survivors in order, *d_count_out their
+ * number.  workspace: b200romp_bev_long_merge_workspace_bytes(capacity) bytes of device memory. */
+long long b200romp_bev_long_merge_workspace_bytes(int capacity);
+int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
+                            const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
+                            float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream);
 /* dst[i] = src[sel[i]] for i < *d_count; rows of row_bytes (multiple of 4) bytes. */
 int b200romp_gather_rows(const void* src, int row_bytes, const int* sel, const int* d_count, int capacity, void* dst,
                          b200romp_stream stream);

@@ -152,6 +152,9 @@ def load():
     _sig(lib.b200romp_bev_parse3d, i32, vp, i32, f32, i32, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_regress, i32, vp, vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_post, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_bev_crop_post, i32, *([vp] * 11), i32, i32, vp, vp, i32, f32, vp, vp, vp, vp, i32, *([vp] * 9), vp)
+    _sig(lib.b200romp_bev_long_merge_workspace_bytes, i64, i32)
+    _sig(lib.b200romp_bev_long_merge, i32, vp, vp, vp, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_gather_rows, i32, vp, i32, vp, vp, i32, vp, vp)
     _sig(lib.b200romp_tracks_create, vp, i32, i32)
     _sig(lib.b200romp_tracks_destroy, None, vp)
@@ -183,6 +186,7 @@ EXPORTS = [
     "b200romp_smpl_workspace_floats", "b200romp_smpl_forward", "b200romp_project",
     "b200romp_bev_create", "b200romp_bev_destroy", "b200romp_bev_bv_input", "b200romp_bev_center3d",
     "b200romp_bev_parse_workspace_bytes", "b200romp_bev_parse3d", "b200romp_bev_regress", "b200romp_bev_post",
+    "b200romp_bev_crop_post", "b200romp_bev_long_merge_workspace_bytes", "b200romp_bev_long_merge",
     "b200romp_gather_rows", "b200romp_pack_rows", "b200romp_preprocess_bgr", "b200romp_tracks_create", "b200romp_tracks_destroy",
     "b200romp_tracks_reset", "b200romp_one_euro_smooth",
 ]

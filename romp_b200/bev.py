@@ -2,7 +2,9 @@
 
 ``bev_settings`` mirrors bev/main.py:27-87 (same flags and defaults, including the quirk that ``crowd`` defaults to
 True and therefore overrides the thresholds with ``long_conf_dict``), ``BEV(settings)(image_bgr) -> dict | None``
-mirrors bev/main.py:91-181 for normal (non-panoramic) images; ``forward_batch`` is the batched entry point.
+mirrors bev/main.py:91-258: normal images run as one 512x512 frame, and in crowd mode images at least twice as wide as
+high run through ``process_long_image`` (the reference's overlapping crops, batched through the model, with the per-crop
+and merged filters on the device).  ``forward_batch`` is the batched entry point for normal frames.
 Per-frame semantics of the two post filters (bev/post_parser.py:167-222) are preserved by applying them per
 ``pred_batch_ids`` group on the device.  Python only allocates buffers and sequences library calls.
 """
@@ -70,8 +72,48 @@ def bev_settings(input_args=sys.argv[1:]):
     return args
 
 
+def long_image_plan(h, w, overlap_ratio):
+    """padding_image_overlap + get_image_split_plan (bev/split2process.py:6-39) for an h x w image.
+
+    Returns (pad_length, boxes int32 [K,4] of [left, right, top, bottom] in the horizontally zero-padded image of width
+    w + 2*pad_length, pad_info6 of the full image).  Same float arithmetic and int32 truncation as the reference,
+    including its last box: left = W - h but the previous box's right, so it is narrower than h."""
+    pad_length = int(h * overlap_ratio)
+    W = w + 2 * pad_length
+    k = int(np.ceil((W / h - 1) / (1 - overlap_ratio))) + 1
+    step = (1 - overlap_ratio) * h
+    boxes, right = [], None
+    for i in range(k):
+        if i == k - 1:
+            left = W - h
+        else:
+            left = step * i
+            right = left + h
+        boxes.append([left, right, 0, h])
+    top = (w - h) // 2
+    return pad_length, np.array(boxes).astype(np.int32), np.array([top, w - top, 0, w, h, w], np.float32)
+
+
+def long_image_crop_table(boxes, pad_length, h, w, nms_thresh):
+    """Per-crop constants of the long-image stages (fp32 [K,6], see b200romp_bev_crop_post): boundary limits
+    (bev/main.py:209-226), projection size and suppression pixels (:216-217,231), cam scale and x shift
+    (split2process.py:48-58; float64 on the host, applied to fp32 like the reference's in-place ops)."""
+    k = len(boxes)
+    tab = np.zeros((k, 6), np.float64)
+    ratio = [(int(boxes[i, 1]) - int(boxes[i + 1, 0])) / h / 2 for i in range(k - 1)]
+    for i, (l, r, t, b) in enumerate(boxes.tolist()):
+        side = max(b - t, r - l)
+        tab[i, 0] = 1 - ratio[i] if i < k - 1 else np.inf
+        tab[i, 1] = ratio[i - 1] - 1 if i >= 2 else -np.inf
+        tab[i, 2] = side
+        tab[i, 3] = nms_thresh * side / 640
+        tab[i, 4] = max(r - l, b - t) / max(h, w)
+        tab[i, 5] = ((l - pad_length) + (r - pad_length)) / 2 / (w / 2) - 1
+    return tab.astype(np.float32)
+
+
 class BEV(torch.nn.Module):
-    """``BEV(settings)(image_bgr)`` - the contract of simple_romp/bev/main.py:91-181 for normal images."""
+    """``BEV(settings)(image_bgr)`` - the contract of simple_romp/bev/main.py:91-258 (normal and crowd-mode images)."""
 
     result_keys = ["smpl_thetas", "smpl_betas", "cam", "cam_trans", "params_pred", "center_confs", "pred_batch_ids"]   # :115
 
@@ -242,11 +284,139 @@ class BEV(torch.nn.Module):
             self.run_post(B, offsets if offsets is not None else [0, 512, 0, 512, 512, 512], img_max_side)
         return self.collect(to_numpy)
 
+    def _long_buffers(self, rows):
+        """Image-level accumulation rows of the long-image mode (grown on demand, kept for the next image)."""
+        lb = getattr(self, "_long", None)
+        if lb is not None and lb["cam"].shape[0] >= rows:
+            return lb
+        dev = self.tdevice
+        z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
+        lb = dict(verts=z(rows, 6890, 3), joints=z(rows, 71, 3), thetas=z(rows, 72), betas=z(rows, 11), params_pred=z(rows, N_PARAMS),
+                  conf=z(rows), cam=z(rows, 3), cam_trans=z(rows, 3), pj2d_org=z(rows, 71, 2), removed=z(rows, dtype=torch.int32),
+                  sel=z(rows, dtype=torch.int32), count=z(2, dtype=torch.int32), count2=z(1, dtype=torch.int32),
+                  ctl=z(2, dtype=torch.int32), cam_full=z(self.cap, 3),
+                  ws=torch.zeros(int(self.lib.b200romp_bev_long_merge_workspace_bytes(rows)), dtype=torch.uint8, device=dev))
+        lb["out"] = {k: torch.zeros_like(lb[k]) for k in ("verts", "joints", "thetas", "betas", "params_pred", "conf", "cam",
+                                                          "cam_trans", "pj2d_org")}
+        self._long = lb
+        return lb
+
+    @torch.no_grad()
+    def process_long_image(self, full_image, center3d_override=None, to_numpy=True):
+        """Crowd mode for images at least twice as wide as high, bev/main.py:184-258 (``BEV.forward`` dispatches here).
+
+        The image is zero-padded horizontally on the device and cut into the reference's overlapping crops
+        (``long_image_plan``); every crop becomes a 512x512 frame (b200romp_preprocess_bgr on the crop's window of the
+        padded image), the crops run through the model in chunks of at most ``max_batch`` frames, each chunk's
+        persons go through the per-crop filters and are appended to image-level rows (b200romp_bev_crop_post), and
+        the merged filters run on those rows (b200romp_bev_long_merge).  One host sync per image.
+        center3d_override: optional device [K,64,128,128] replacing the crops' 3-D centre maps (tests, measurement)."""
+        if not self.calc_smpl:
+            raise ValueError("the long-image mode needs SMPL (bev/main.py:203): calc_smpl must be on for images with w/h >= 2")
+        img = torch.from_numpy(np.ascontiguousarray(full_image)) if isinstance(full_image, np.ndarray) else full_image
+        assert img.dtype == torch.uint8 and img.dim() == 3 and img.shape[2] == 3, "image must be HxWx3 uint8 (BGR)"
+        s = self.settings
+        h, w = int(img.shape[0]), int(img.shape[1])
+        pad_length, boxes, pad_info = long_image_plan(h, w, s.overlap_ratio)
+        K, B = len(boxes), self.max_batch
+        if center3d_override is not None:
+            assert center3d_override.is_cuda and tuple(center3d_override.shape) == (K, 64, 128, 128)
+            cur = torch.cuda.current_stream(self.tdevice)
+            if cur != self.stream:
+                self.stream.wait_stream(cur)
+            center3d_override.record_stream(self.stream)
+        lb = self._long_buffers(K * MAX_PERSON)
+        tab = torch.from_numpy(long_image_crop_table(boxes, pad_length, h, w, float(s.nms_thresh))).pin_memory()
+        key = (torch.uint8, B)
+        if key not in self._staging:
+            self._staging[key] = torch.empty((B, 512, 512, 3), dtype=torch.uint8, device=self.tdevice)
+        frames = self._staging[key]
+        with torch.cuda.stream(self.stream):
+            padded = self.pad_long_image(img, pad_length)
+            tab_dev = tab.to(self.tdevice, non_blocking=True)
+            lb["count"].zero_()
+            for c0 in range(0, K, B):
+                nb = min(B, K - c0)
+                self.crop_frames(padded, boxes[c0:c0 + nb], frames)                         # main.py:197-199 + img_preprocess
+                self.run_model(frames[:nb], None if center3d_override is None else center3d_override[c0:c0 + nb])
+                self.crop_post(nb, c0, tab_dev)
+            self.long_merge(pad_info, w)
+        return self._collect_long(to_numpy)
+
+    def pad_long_image(self, img, pad_length):
+        """padding_image_overlap (split2process.py:6-13) on the device: h x (w + 2*pad_length) x 3, zero columns each side."""
+        h, w = int(img.shape[0]), int(img.shape[1])
+        raw = img if img.is_cuda else img.to(self.tdevice, non_blocking=True)
+        padded = torch.zeros((h, w + 2 * pad_length, 3), dtype=torch.uint8, device=self.tdevice)
+        padded[:, pad_length:pad_length + w] = raw
+        return padded
+
+    def crop_frames(self, padded, boxes, frames):
+        """frames[i] = img_preprocess(padded[t:b, l:r]) for box i: one b200romp_preprocess_bgr per crop on its window of the
+        padded image (pointer offset, the crop's own size, the padded row stride)."""
+        W, sp = int(padded.shape[1]), C.c_void_p(self.stream.cuda_stream)
+        for i, (l, r, t, b) in enumerate(np.asarray(boxes).tolist()):
+            _lib.check(self.lib.b200romp_preprocess_bgr(C.c_void_p(padded.data_ptr() + (t * W + l) * 3), b - t, r - l, 3 * W, 512,
+                                                        C.c_void_p(frames[i].data_ptr()), None, sp), "preprocess_bgr")
+
+    def crop_post(self, nb, crop0, tab_dev):
+        """SMPL-A / SMIL on the chunk's persons, then the per-crop stage (b200romp_bev_crop_post): survivors appended to
+        the image-level rows."""
+        lib, b, lb, st = self.lib, self.buf, self._long, self.stream.cuda_stream
+        cap = nb * MAX_PERSON
+        self.smpla.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts"], b["joints"], st)
+        self.smil.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts_smil"], b["joints_smil"], st)
+        _lib.check(lib.b200romp_bev_crop_post(
+            _ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]), _ptr(b["joints"]),
+            _ptr(b["thetas"]), _ptr(b["params_pred"]), _ptr(b["conf"]), _ptr(b["cam"]), _ptr(b["cam_trans"]),
+            _ptr(b["batch_ids"]), nb, cap, _ptr(b["count"]), _ptr(tab_dev), crop0, float(self.settings.relative_scale_thresh),
+            _ptr(b["pj2d_org"]), _ptr(b["keep"]), _ptr(b["sel"]), _ptr(lb["cam_full"]), lb["cam"].shape[0], _ptr(lb["count"]),
+            _ptr(lb["ctl"]), _ptr(lb["verts"]), _ptr(lb["joints"]), _ptr(lb["thetas"]), _ptr(lb["betas"]),
+            _ptr(lb["params_pred"]), _ptr(lb["conf"]), _ptr(lb["cam"]), C.c_void_p(st)), "bev_crop_post")
+
+    @torch.no_grad()
+    def long_merge(self, pad_info, img_max_side):
+        """Merged stage of the long-image mode (bev/main.py:253-256) on the accumulated rows, then row compaction."""
+        lib, lb, sp = self.lib, self._long, C.c_void_p(self.stream.cuda_stream)
+        rows = lb["cam"].shape[0]
+        off = (C.c_float * 6)(*[float(v) for v in pad_info])
+        _lib.check(lib.b200romp_bev_long_merge(_ptr(lb["cam"]), _ptr(lb["joints"]), _ptr(lb["conf"]), rows, _ptr(lb["count"]), off,
+                                               float(self.settings.nms_thresh), float(self.settings.relative_scale_thresh),
+                                               float(img_max_side), _ptr(lb["cam_trans"]), _ptr(lb["pj2d_org"]), _ptr(lb["removed"]),
+                                               _ptr(lb["ws"]), _ptr(lb["sel"]), _ptr(lb["count2"]), sp), "bev_long_merge")
+        for k, dst in lb["out"].items():
+            src = lb[k]
+            row = src[0].numel() * src.element_size()
+            _lib.check(lib.b200romp_gather_rows(_ptr(src), row, _ptr(lb["sel"]), _ptr(lb["count2"]), rows, _ptr(dst), sp), "gather_rows")
+
+    def _collect_long(self, to_numpy=True):
+        lb = self._long
+        with torch.cuda.stream(self.stream):
+            self.count_host[0:1].copy_(lb["count"][1:2], non_blocking=True)            # persons detected in any crop
+            self.count_host[1:2].copy_(lb["count2"], non_blocking=True)
+        self.stream.synchronize()
+        n_det, n = int(self.count_host[0]), int(self.count_host[1])
+        if n_det == 0:                        # the reference raises KeyError here (main.py:253); INTEGRATION.md, Deviations
+            print("No person detected!")
+            return None
+        o = lb["out"]
+        out = {"smpl_thetas": o["thetas"][:n], "smpl_betas": o["betas"][:n], "cam": o["cam"][:n], "cam_trans": o["cam_trans"][:n],
+               "params_pred": o["params_pred"][:n], "center_confs": o["conf"][:n],
+               "pred_batch_ids": torch.zeros(n, dtype=torch.int64, device=self.tdevice),
+               "verts": o["verts"][:n], "joints": o["joints"][:n], "pj2d_org": o["pj2d_org"][:n]}
+        if to_numpy:
+            with torch.cuda.stream(self.stream):
+                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
+        return out
+
     @torch.no_grad()
     def forward(self, image, signal_ID=0, **kwargs):
-        """image: HxWx3 uint8 BGR.  bev/main.py:139-156 (normal images; the >=2:1 panoramic tiling is out of scope)."""
+        """image: HxWx3 uint8 BGR.  bev/main.py:139-156: crowd mode (the default) takes images with w/h >= 2 through
+        ``process_long_image``, every other image through one 512x512 frame."""
         if image.shape[1] / image.shape[0] >= 2 and self.settings.crowd:
-            raise NotImplementedError("long-image sliding-window processing (bev/split2process.py) is out of scope")
+            if getattr(self.settings, "show_patch_results", False):
+                raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
+            return self.process_long_image(image)
         inp, pad = img_preprocess(image)
         out = self.forward_batch(torch.from_numpy(inp), offsets=pad, img_max_side=float(max(image.shape[:2])))
         if out is None:

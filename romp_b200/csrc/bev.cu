@@ -386,31 +386,32 @@ __global__ void __launch_bounds__(128) bev_project_kernel(const float* __restric
   pj2d_org[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f - top;
 }
 
-// one CTA per frame: both reference post-filters on that frame's (<= 64) persons, then flags for the survivors
-__global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
-                                                             const float* __restrict__ cam_trans, const long long* __restrict__ batch_ids,
-                                                             const int* __restrict__ d_count, float nms_thr_px, float rel_scale_thresh,
-                                                             int* __restrict__ keep) {
-  __shared__ int s_start, s_n;
-  __shared__ int s_removed[kMaxP], s_kept[kMaxP], s_nk;
-  __shared__ float s_mean[kMaxP];
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int N = *d_count;
-  if (tid == 0) {
-    int s = 0;
-    while (s < N && batch_ids[s] < b) ++s;
-    int e = s;
-    while (e < N && batch_ids[e] == b) ++e;
-    s_start = s; s_n = min(e - s, kMaxP);
-  }
-  if (tid < kMaxP) s_removed[tid] = 0;
+// [start, start + n) = the rows of frame b (rows are grouped by frame, in frame order); n capped at 64
+__device__ __forceinline__ void frame_rows(const long long* __restrict__ batch_ids, int N, int b, int* s_start, int* s_n) {
+  int s = 0;
+  while (s < N && batch_ids[s] < b) ++s;
+  int e = s;
+  while (e < N && batch_ids[e] == b) ++e;
+  *s_start = s; *s_n = min(e - s, kMaxP);
+}
+
+// Both reference post-filters on one frame's (<= 64) persons [st, st + nf), by the whole CTA (256 threads).  Persons with
+// s_drop[i] set on entry take part in neither filter (the long-image boundary drop).  On return s_removed[i] = 1 for every
+// person that is dropped or filtered out.
+//   suppressing_redundant_prediction_via_projection (bev/post_parser.py:167-198): every pair below the threshold at once;
+//     conf == nullptr removes the smaller scale (cam[:,0]) of the pair, else the lower center_confs (conf_based=True, :191-193);
+//     on a tie the later person
+//   remove_outlier(relative_scale_thresh, scale_thresh) (:200-222)
+__device__ void postfilter_frame(const float* __restrict__ pj2d_org, const float* __restrict__ cam, const float* __restrict__ cam_trans,
+                                 const float* __restrict__ conf, int st, int nf, float nms_thr_px, float rel_scale_thresh,
+                                 float scale_thresh, const int* s_drop, int* s_removed, int* s_kept, float* s_mean, int* s_nk) {
+  const int tid = threadIdx.x;
+  if (tid < kMaxP) s_removed[tid] = tid < nf ? s_drop[tid] : 0;
   __syncthreads();
-  const int st = s_start, nf = s_n;
-  if (nf == 0) return;
-  if (nf > 1) {       // suppressing_redundant_prediction_via_projection, bev/post_parser.py:167-198
-    for (int pr = tid; pr < nf * nf; pr += 256) {
+  if (nf > 1) {
+    for (int pr = tid; pr < nf * nf; pr += blockDim.x) {
       const int i = pr / nf, j = pr % nf;
-      if (i >= j) continue;
+      if (i >= j || s_drop[i] || s_drop[j]) continue;
       const float* a = pj2d_org + (size_t)(st + i) * 142;
       const float* c = pj2d_org + (size_t)(st + j) * 142;
       float sum = 0.f;
@@ -419,7 +420,10 @@ __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __rest
         sum += sqrtf(dx * dx + dy * dy);
       }
       const float si = cam[(st + i) * 3] * 2.f, sj = cam[(st + j) * 3] * 2.f;
-      if (sum / 71.f / fmaxf(si, sj) < nms_thr_px) atomicExch(&s_removed[si < sj ? i : j], 1);
+      if (sum / 71.f / fmaxf(si, sj) < nms_thr_px) {
+        const bool first = conf ? conf[st + i] < conf[st + j] : si < sj;
+        atomicExch(&s_removed[first ? i : j], 1);
+      }
     }
   }
   __syncthreads();
@@ -427,11 +431,11 @@ __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __rest
     int k = 0;
     for (int i = 0; i < nf; ++i)
       if (!s_removed[i]) s_kept[k++] = i;
-    s_nk = k;
+    *s_nk = k;
   }
   __syncthreads();
-  const int nk = s_nk;
-  if (nk >= 3) {      // remove_outlier, bev/post_parser.py:200-222
+  const int nk = *s_nk;
+  if (nk >= 3) {
     if (tid < nk) {
       const float* ti = cam_trans + (size_t)(st + s_kept[tid]) * 3;
       float sum = 0.f, mn = CUDART_INF_F, mx = -CUDART_INF_F;
@@ -448,11 +452,255 @@ __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __rest
       float tot = 0.f;
       for (int j = 0; j < nk; ++j) tot += s_mean[j];
       const float rel = s_mean[tid] / ((tot - s_mean[tid]) / (float)(nk - 1));
-      if (rel > rel_scale_thresh && cam[(st + s_kept[tid]) * 3] < 0.25f) s_removed[s_kept[tid]] = 1;
+      if (rel > rel_scale_thresh && cam[(st + s_kept[tid]) * 3] < scale_thresh) s_removed[s_kept[tid]] = 1;
     }
     __syncthreads();
   }
+}
+
+// one CTA per frame: both reference post-filters on that frame's (<= 64) persons, then flags for the survivors
+__global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
+                                                             const float* __restrict__ cam_trans, const long long* __restrict__ batch_ids,
+                                                             const int* __restrict__ d_count, float nms_thr_px, float rel_scale_thresh,
+                                                             int* __restrict__ keep) {
+  __shared__ int s_start, s_n;
+  __shared__ int s_drop[kMaxP], s_removed[kMaxP], s_kept[kMaxP], s_nk;
+  __shared__ float s_mean[kMaxP];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n);
+  if (tid < kMaxP) s_drop[tid] = 0;
+  __syncthreads();
+  const int st = s_start, nf = s_n;
+  if (nf == 0) return;
+  postfilter_frame(pj2d_org, cam, cam_trans, nullptr, st, nf, nms_thr_px, rel_scale_thresh, 0.25f, s_drop, s_removed, s_kept, s_mean, &s_nk);
   if (tid < nf) keep[st + tid] = s_removed[tid] ? 0 : 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Long-image (crowd) mode, bev/main.py:184-258.  Per-crop table row (fp32, one per crop of the image):
+//   [0] drop persons with cam x > this (1 - ratio(i), +inf for the last crop)             main.py:209-215, split2process.py:41-46
+//   [1] drop persons with cam x < this (ratio(i-1) - 1 for crops 2.., -inf for crops 0, 1)  :221-226
+//   [2] projection size max(ch, cw) (offsets [0, ch, 0, cw, ch, cw])                        :216-217
+//   [3] suppression threshold in pixels, nms_thresh * max(ch, cw) / 640                      :231
+//   [4] cam scale max(r-l, b-t) / max(h, w), [5] cam x shift mean(l, r) / (w/2) - 1          split2process.py:48-58
+constexpr int kCropTab = 6;
+
+// one CTA per crop of the chunk: boundary drop, projection to crop pixels, conf-based suppression, remove_outlier with
+// scale_thresh 1, then keep flags and the full-image cam of every person
+__global__ void __launch_bounds__(256) bev_crop_filter_kernel(const float* __restrict__ joints, const float* __restrict__ cam,
+                                                              const float* __restrict__ cam_trans, const float* __restrict__ conf,
+                                                              const long long* __restrict__ batch_ids, const int* __restrict__ d_count,
+                                                              const float* __restrict__ crop_table, int crop0, float rel_scale_thresh,
+                                                              float* __restrict__ pj2d, int* __restrict__ keep,
+                                                              float* __restrict__ cam_full) {
+  __shared__ int s_start, s_n;
+  __shared__ int s_drop[kMaxP], s_removed[kMaxP], s_kept[kMaxP], s_nk;
+  __shared__ float s_mean[kMaxP];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n);
+  __syncthreads();
+  const int st = s_start, nf = s_n;
+  if (nf == 0) return;
+  const float* tab = crop_table + (size_t)(crop0 + b) * kCropTab;
+  if (tid < nf) {
+    const float x = cam[(st + tid) * 3 + 2];
+    s_drop[tid] = (x > tab[0] || x < tab[1]) ? 1 : 0;
+  }
+  const float size = tab[2];
+  for (int t = tid; t < nf * 71; t += 256) {       // perspective_projection + convert_proejection_from_input_to_orgimg
+    const int n = st + t / 71, j = t % 71;
+    const float* q = joints + ((size_t)n * 71 + j) * 3;
+    const float px = q[0] + cam_trans[n * 3], py = q[1] + cam_trans[n * 3 + 1], pz = q[2] + cam_trans[n * 3 + 2];
+    const float iz = pz + 1e-6f;
+    const float u = (px / iz) * 443.4f / 256.f, v = (py / iz) * 443.4f / 256.f;
+    pj2d[((size_t)n * 71 + j) * 2 + 0] = (u + 1.f) * size / 2.f;
+    pj2d[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f;
+  }
+  __syncthreads();
+  postfilter_frame(pj2d, cam, cam_trans, conf, st, nf, tab[3], rel_scale_thresh, 1.f, s_drop, s_removed, s_kept, s_mean, &s_nk);
+  if (tid < nf) {
+    const int n = st + tid;
+    keep[n] = s_removed[tid] ? 0 : 1;
+    // convert_crop_cam_params2full_image: cam *= scale (all three), then cam[:,2] += shift, fp32 like the in-place torch ops
+    const float s = tab[4];
+    cam_full[n * 3 + 0] = __fmul_rn(cam[n * 3 + 0], s);
+    cam_full[n * 3 + 1] = __fmul_rn(cam[n * 3 + 1], s);
+    cam_full[n * 3 + 2] = __fadd_rn(__fmul_rn(cam[n * 3 + 2], s), tab[5]);
+  }
+}
+
+// Stable compaction by one CTA (blockDim a multiple of 32, <= 1024): out[k] = val(i) for the k-th i < n with flag(i); returns
+// the count to every thread.
+template <class Flag, class Val>
+__device__ int block_compact(int n, Flag flag, Val val, int* __restrict__ out) {
+  __shared__ int s_warp[32], s_base, s_tot;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
+  if (tid == 0) s_base = 0;
+  __syncthreads();
+  for (int c = 0; c < n; c += blockDim.x) {
+    const int i = c + tid;
+    const bool f = i < n && flag(i);
+    const unsigned m = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) s_warp[wid] = __popc(m);
+    __syncthreads();
+    if (wid == 0) {
+      const int v = lane < nw ? s_warp[lane] : 0;
+      int inc = v;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += u;
+      }
+      if (lane < nw) s_warp[lane] = inc - v;
+      if (lane == 31) s_tot = inc;
+    }
+    __syncthreads();
+    if (f) out[s_base + s_warp[wid] + __popc(m & ((1u << lane) - 1u))] = val(i);
+    __syncthreads();
+    if (tid == 0) s_base += s_tot;
+    __syncthreads();
+  }
+  return s_base;
+}
+
+// append the chunk's survivors at the image's running count acc_count[0]: sel = their chunk rows, ctl = {base, n_new}
+__global__ void __launch_bounds__(1024) bev_crop_append_kernel(const int* __restrict__ keep, const int* __restrict__ d_count,
+                                                               int acc_capacity, int* __restrict__ acc_count, int* __restrict__ sel,
+                                                               int* __restrict__ ctl) {
+  const int N = *d_count;
+  const int k = block_compact(N, [&](int i) { return keep[i] != 0; }, [](int i) { return i; }, sel);
+  if (threadIdx.x == 0) {
+    const int base = *acc_count, n = min(k, acc_capacity - base);
+    ctl[0] = base; ctl[1] = n;
+    acc_count[0] = base + n;
+    acc_count[1] += N;                    // persons detected in the image so far, survivors or not
+  }
+}
+
+__global__ void __launch_bounds__(256) append_rows_kernel(const uint32_t* __restrict__ src, int row_words, const int* __restrict__ sel,
+                                                          const int* __restrict__ ctl, uint32_t* __restrict__ dst) {
+  const int i = blockIdx.x;
+  if (i >= ctl[1]) return;
+  const uint32_t* s = src + (size_t)sel[i] * row_words;
+  uint32_t* d = dst + (size_t)(ctl[0] + i) * row_words;
+  for (int k = blockIdx.y * 256 + threadIdx.x; k < row_words; k += gridDim.y * 256) d[k] = s[k];
+}
+
+// merged stage, bev/main.py:253-256: cam_trans from the full-image cam and projection with the full image's pad info
+__global__ void __launch_bounds__(128) bev_long_project_kernel(const float* __restrict__ cam, const float* __restrict__ joints,
+                                                               const int* __restrict__ d_count, float size, float left, float top,
+                                                               float* __restrict__ cam_trans, float* __restrict__ pj2d_org,
+                                                               int* __restrict__ removed) {
+  const int n = blockIdx.x, j = threadIdx.x;
+  if (n >= *d_count) return;
+  // denormalize_cam_params_to_trans (bev/post_parser.py:114-128), rounded op by op like the torch ops
+  const float depth = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(cam[n * 3], kTanFov), 1e-3f));
+  const float tx = __fmul_rn(__fmul_rn(cam[n * 3 + 2], depth), kTanFov), ty = __fmul_rn(__fmul_rn(cam[n * 3 + 1], depth), kTanFov);
+  if (j == 0) {
+    cam_trans[n * 3 + 0] = tx; cam_trans[n * 3 + 1] = ty; cam_trans[n * 3 + 2] = depth;
+    removed[n] = 0;
+  }
+  if (j >= 71) return;
+  const float* q = joints + ((size_t)n * 71 + j) * 3;
+  const float iz = q[2] + depth + 1e-6f;
+  const float u = ((q[0] + tx) / iz) * 443.4f / 256.f, v = ((q[1] + ty) / iz) * 443.4f / 256.f;
+  pj2d_org[((size_t)n * 71 + j) * 2 + 0] = (u + 1.f) * size / 2.f - left;
+  pj2d_org[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f - top;
+}
+
+// conf-based suppression over ALL accumulated persons (not bounded by 64): one 16 x 16 tile of pairs (i < j) per CTA; every
+// pair below the threshold removes its lower-confidence member, all pairs at once like the reference's torch.where
+constexpr int kPT = 16;
+__global__ void __launch_bounds__(256) bev_long_pairs_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
+                                                             const float* __restrict__ conf, const int* __restrict__ d_count,
+                                                             float nms_thr_px, int* __restrict__ removed) {
+  __shared__ float s_a[kPT][142], s_b[kPT][142];
+  const int N = *d_count;
+  const int i0 = blockIdx.y * kPT, j0 = blockIdx.x * kPT;
+  if (i0 >= N || j0 >= N || j0 + kPT - 1 <= i0) return;
+  for (int t = threadIdx.x; t < kPT * 142; t += 256) {
+    const int r = t / 142, c = t % 142;
+    s_a[r][c] = i0 + r < N ? pj2d_org[(size_t)(i0 + r) * 142 + c] : 0.f;
+    s_b[r][c] = j0 + r < N ? pj2d_org[(size_t)(j0 + r) * 142 + c] : 0.f;
+  }
+  __syncthreads();
+  const int ii = threadIdx.x / kPT, jj = threadIdx.x % kPT, i = i0 + ii, j = j0 + jj;
+  if (i >= N || j >= N || i >= j) return;
+  float sum = 0.f;
+  for (int k = 0; k < 71; ++k) {
+    const float dx = s_a[ii][2 * k] - s_b[jj][2 * k], dy = s_a[ii][2 * k + 1] - s_b[jj][2 * k + 1];
+    sum += sqrtf(dx * dx + dy * dy);
+  }
+  const float si = cam[i * 3] * 2.f, sj = cam[j * 3] * 2.f;
+  if (sum / 71.f / fmaxf(si, sj) < nms_thr_px) removed[conf[i] < conf[j] ? i : j] = 1;
+}
+
+// survivors of the suppression: ws_sel[0, nk), *ws_nk = nk
+__global__ void __launch_bounds__(1024) bev_long_kept_kernel(const int* __restrict__ removed, const int* __restrict__ d_count,
+                                                             int* __restrict__ ws_sel, int* __restrict__ ws_nk) {
+  const int k = block_compact(*d_count, [&](int i) { return removed[i] == 0; }, [](int i) { return i; }, ws_sel);
+  if (threadIdx.x == 0) *ws_nk = k;
+}
+
+// remove_outlier, mean of each survivor's sorted distance row without its first and last entry: one CTA per survivor
+__global__ void __launch_bounds__(128) bev_long_meandist_kernel(const float* __restrict__ cam_trans, const int* __restrict__ ws_sel,
+                                                                const int* __restrict__ ws_nk, float* __restrict__ ws_mean) {
+  const int nk = *ws_nk, r = blockIdx.x;
+  if (nk < 3 || r >= nk) return;
+  const float* ti = cam_trans + (size_t)ws_sel[r] * 3;
+  float sum = 0.f, mn = CUDART_INF_F, mx = -CUDART_INF_F;
+  for (int k = threadIdx.x; k < nk; k += 128) {
+    const float* tj = cam_trans + (size_t)ws_sel[k] * 3;
+    const float dx = ti[0] - tj[0], dy = ti[1] - tj[1], dz = ti[2] - tj[2];
+    const float d = sqrtf(dx * dx + dy * dy + dz * dz);
+    sum += d; mn = fminf(mn, d); mx = fmaxf(mx, d);
+  }
+  __shared__ float s_sum[4], s_mn[4], s_mx[4];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = sum; s_mn[threadIdx.x >> 5] = mn; s_mx[threadIdx.x >> 5] = mx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const float s = s_sum[0] + s_sum[1] + s_sum[2] + s_sum[3];
+    const float lo = fminf(fminf(s_mn[0], s_mn[1]), fminf(s_mn[2], s_mn[3])), hi = fmaxf(fmaxf(s_mx[0], s_mx[1]), fmaxf(s_mx[2], s_mx[3]));
+    ws_mean[r] = (s - lo - hi) / (float)(nk - 2);
+  }
+}
+
+// relative scale of every survivor against the others, outliers (and cam[:,0] < scale_thresh) removed, final compaction
+__global__ void __launch_bounds__(1024) bev_long_outlier_kernel(const float* __restrict__ cam, const int* __restrict__ ws_sel,
+                                                                const int* __restrict__ ws_nk, const float* __restrict__ ws_mean,
+                                                                float rel_scale_thresh, float scale_thresh, int* __restrict__ sel,
+                                                                int* __restrict__ d_count_out) {
+  __shared__ float s_part[32];
+  __shared__ float s_tot;
+  const int nk = *ws_nk, tid = threadIdx.x;
+  float tot = 0.f;
+  if (nk >= 3) {
+    for (int k = tid; k < nk; k += blockDim.x) tot += ws_mean[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
+    if ((tid & 31) == 0) s_part[tid >> 5] = tot;
+    __syncthreads();
+    if (tid == 0) {
+      float t = 0.f;
+      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_part[w];
+      s_tot = t;
+    }
+    __syncthreads();
+    tot = s_tot;
+  }
+  auto keep = [&](int k) {
+    if (nk < 3) return true;
+    const float rel = ws_mean[k] / ((tot - ws_mean[k]) / (float)(nk - 1));
+    return !(rel > rel_scale_thresh && cam[ws_sel[k] * 3] < scale_thresh);
+  };
+  const int n = block_compact(nk, keep, [&](int k) { return ws_sel[k]; }, sel);
+  if (tid == 0) *d_count_out = n;
 }
 
 __global__ void bev_compact_kernel(const int* __restrict__ keep, const int* __restrict__ d_count, int* __restrict__ sel,
@@ -620,6 +868,56 @@ int b200romp_bev_post(const float* betas, const float* verts_smil, const float* 
   bev_postfilter_kernel<<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
                                                    rel_scale_thresh, keep);
   bev_compact_kernel<<<1, 32, 0, stream>>>(keep, d_count, sel, d_count_out);
+  B2R_CUDA_OK(cudaGetLastError());
+  return B200ROMP_OK;
+}
+
+int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                           const float* thetas, const float* params_pred, const float* conf, const float* cam, const float* cam_trans,
+                           const long long* batch_ids, int batch, int capacity, const int* d_count, const float* crop_table,
+                           int crop0, float rel_scale_thresh, float* pj2d, int* keep, int* sel, float* cam_full, int acc_capacity,
+                           int* acc_count, int* acc_ctl, float* acc_verts, float* acc_joints, float* acc_thetas, float* acc_betas,
+                           float* acc_params_pred, float* acc_conf, float* acc_cam, b200romp_stream stream_) {
+  B2R_REQUIRE(betas && verts && joints && thetas && params_pred && conf && cam && cam_trans && batch_ids && d_count && crop_table &&
+                  pj2d && keep && sel && cam_full && acc_count && acc_ctl && acc_verts && acc_joints && acc_thetas && acc_betas &&
+                  acc_params_pred && acc_conf && acc_cam && batch > 0 && capacity > 0 && crop0 >= 0 && acc_capacity > 0,
+              "bev_crop_post: bad arguments");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (verts_smil && joints_smil)
+    bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
+  B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
+  bev_crop_filter_kernel<<<batch, 256, 0, stream>>>(joints, cam, cam_trans, conf, batch_ids, d_count, crop_table, crop0,
+                                                    rel_scale_thresh, pj2d, keep, cam_full);
+  bev_crop_append_kernel<<<1, 1024, 0, stream>>>(keep, d_count, acc_capacity, acc_count, sel, acc_ctl);
+  const struct { const void* src; void* dst; int words; } rows[] = {
+      {verts, acc_verts, 6890 * 3}, {joints, acc_joints, 71 * 3}, {thetas, acc_thetas, 72}, {betas, acc_betas, 11},
+      {params_pred, acc_params_pred, 146}, {conf, acc_conf, 1}, {cam_full, acc_cam, 3}};
+  for (const auto& r : rows)
+    append_rows_kernel<<<dim3(capacity, r.words > 4096 ? 8 : 1), 256, 0, stream>>>(
+        reinterpret_cast<const uint32_t*>(r.src), r.words, sel, acc_ctl, reinterpret_cast<uint32_t*>(r.dst));
+  B2R_CUDA_OK(cudaGetLastError());
+  return B200ROMP_OK;
+}
+
+long long b200romp_bev_long_merge_workspace_bytes(int capacity) { return (long long)capacity * 8 + 16; }
+
+int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
+                            const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
+                            float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream_) {
+  B2R_REQUIRE(cam && joints && conf && d_count && offsets6 && cam_trans && pj2d_org && removed && workspace && sel && d_count_out &&
+                  capacity > 0 && img_max_side > 0.f, "bev_long_merge: bad arguments");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int* ws_nk = reinterpret_cast<int*>(workspace);
+  int* ws_sel = ws_nk + 4;
+  float* ws_mean = reinterpret_cast<float*>(ws_sel + capacity);
+  const float top = offsets6[0], left = offsets6[2], hh = offsets6[4], ww = offsets6[5];
+  bev_long_project_kernel<<<capacity, 128, 0, stream>>>(cam, joints, d_count, hh > ww ? hh : ww, left, top, cam_trans, pj2d_org, removed);
+  const unsigned tiles = (unsigned)((capacity + kPT - 1) / kPT);
+  bev_long_pairs_kernel<<<dim3(tiles, tiles), 256, 0, stream>>>(pj2d_org, cam, conf, d_count,
+                                                                (float)((double)nms_thresh * img_max_side / 640.0), removed);
+  bev_long_kept_kernel<<<1, 1024, 0, stream>>>(removed, d_count, ws_sel, ws_nk);
+  bev_long_meandist_kernel<<<capacity, 128, 0, stream>>>(cam_trans, ws_sel, ws_nk, ws_mean);
+  bev_long_outlier_kernel<<<1, 1024, 0, stream>>>(cam, ws_sel, ws_nk, ws_mean, rel_scale_thresh, 0.5f, sel, d_count_out);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
 }
