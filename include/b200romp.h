@@ -33,7 +33,8 @@ enum { B200ROMP_F32 = 0, B200ROMP_BF16 = 1, B200ROMP_U8 = 2 };
 /* AUTO: bf16 tensors -> tensor cores (wgmma bf16), fp32 tensors -> SIMT fp32.  TF32: fp32 tensors -> wgmma tf32 (operands
  * rounded to TF32 with cvt.rna like the reference's cuDNN TF32 convs, fp32 accumulate, fp32 tensors in HBM) where the
  * shape tiles onto the engine, SIMT fp32 otherwise. */
-enum { B200ROMP_ENGINE_AUTO = 0, B200ROMP_ENGINE_SIMT = 1, B200ROMP_ENGINE_TCGEN05 = 2, B200ROMP_ENGINE_TF32 = 3 };
+enum { B200ROMP_ENGINE_AUTO = 0, B200ROMP_ENGINE_SIMT = 1, B200ROMP_ENGINE_WGMMA = 2, B200ROMP_ENGINE_TF32 = 3 };
+#define B200ROMP_ENGINE_TCGEN05 B200ROMP_ENGINE_WGMMA   /* former name, kept for existing callers */
 
 typedef struct b200romp_net b200romp_net;    /* a conv graph: backbone + heads                          */
 typedef struct b200romp_smpl b200romp_smpl;  /* packed SMPL constants                                     */

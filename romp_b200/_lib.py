@@ -17,7 +17,8 @@ CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "resnet_ops.cu"]
 
 F32, BF16, U8 = 0, 1, 2
-ENGINE_AUTO, ENGINE_SIMT, ENGINE_TCGEN05, ENGINE_TF32 = 0, 1, 2, 3
+ENGINE_AUTO, ENGINE_SIMT, ENGINE_WGMMA, ENGINE_TF32 = 0, 1, 2, 3
+ENGINE_TCGEN05 = ENGINE_WGMMA   # former name, kept for existing callers
 
 
 class ConvDesc(C.Structure):

@@ -170,13 +170,15 @@ int tc_conv1d_prepare(const ConvParams& p, const float* w_oi3, int sm_count, TcC
   B2R_CUDA_OK(cudaMalloc(&plan->d_wpack, img.size() * sizeof(__nv_bfloat16)));
   allocs->push_back(plan->d_wpack);
   B2R_CUDA_OK(cudaMemcpy(plan->d_wpack, img.data(), img.size() * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice));
-  int rc = conv1d_encode(p, plan);
-  if (rc) return rc;
+  if (!tc_get_encode()) {   // resolved now rather than at the first launch, which may be inside a stream capture
+    set_error("conv1d_tc: cuTensorMapEncodeTiled is unavailable");
+    return B200ROMP_ECUDA;
+  }
   return nt == 64 ? conv1d_inst<64>(*plan, p, nullptr, true) : conv1d_inst<32>(*plan, p, nullptr, true);
 }
 
-// the input of the bird's-eye graph is an EXTERNAL tensor (assembled by b200romp_bev_bv_input): re-encode the tensor map
-// when the bound pointer (or the batch) differs from the one the map was built for
+// the input of the bird's-eye graph is an EXTERNAL tensor (assembled by b200romp_bev_bv_input): the tensor map is encoded
+// at the first launch and again whenever the bound pointer (or the batch) differs from the one it was built for
 int tc_conv1d_launch(TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) {
   if (plan.encoded_in != p.in || plan.encoded_batch != p.B) {
     int rc = conv1d_encode(p, &plan);

@@ -248,12 +248,8 @@ bool tc_block_supported(const ConvParams& p) {
   return (reinterpret_cast<uintptr_t>(p.in) & 15) == 0;
 }
 
-int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, bool fold, int sm_count,
+int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
                      TcConvPlan* plan, std::vector<void*>* allocs) {
-  if (!tc_block_supported(p)) {
-    set_error("conv_block_tc: unsupported block shape");
-    return B200ROMP_EINVAL;
-  }
   PFN_encodeTiled encode = tc_get_encode();
   if (!encode) {
     set_error("conv_block_tc: cuTensorMapEncodeTiled is unavailable");
@@ -266,7 +262,6 @@ int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1,
   plan->grid_y = 1;
   plan->stages = 1;
   plan->smem_bytes = kSmemBytes;
-  plan->fold = fold ? 1 : 0;
   int rc = tc_pack_weights(w1_oihw, 64, 64, 9, 64, &plan->d_wpack, allocs, kRowB, 2);
   if (rc) return rc;
   rc = tc_pack_weights(w2_oihw, 64, 64, 9, 64, &plan->d_wpack2, allocs, kRowB, 2);

@@ -171,8 +171,7 @@ bool tc_stem_supported(const ConvParams& p, int ksize, int stride) {
          p.Hout * 2 == p.Hin && p.Wout * 2 == p.Win && (p.Win * 3) % 16 == 0;
 }
 
-int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, bool /*out_final*/, TcConvPlan* plan,
-                    std::vector<void*>* allocs) {
+int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, TcConvPlan* plan, std::vector<void*>* allocs) {
   // weights as a 64 x 32 K-major matrix, k = r*9 + s*3 + c, scaled by 2/255 (the normalisation), zero padded
   std::vector<float> wk((size_t)64 * kStemK, 0.f);
   for (int co = 0; co < 64; ++co)

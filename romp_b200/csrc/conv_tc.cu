@@ -285,7 +285,7 @@ static bool tc_s2_supported(const ConvParams& p) {
   return true;
 }
 
-bool tc_conv_supported(const ConvParams& p, int ksize, int stride) {
+static bool tc_shape_supported(const ConvParams& p, int ksize, int stride) {
   if (stride == 2 && ksize == 3) return tc_s2_supported(p);
   if (stride != 1 || (ksize != 1 && ksize != 3)) return false;
   if ((p.in_dtype != B200ROMP_BF16 && p.in_dtype != B200ROMP_F32) || p.input_norm) return false;   // F32 = the TF32 engine
@@ -302,6 +302,45 @@ bool tc_conv_supported(const ConvParams& p, int ksize, int stride) {
   if (p.res != nullptr && (p.res_C % 8 != 0 || p.res_c_off % 8 != 0)) return false;
   if ((reinterpret_cast<uintptr_t>(p.in) & 15) != 0) return false;
   return true;
+}
+
+static int tc_rowb(int ksize, int stride, int cin, int eb) { return stride == 2 ? s2_row_bytes(cin, eb) : tc_row_bytes(ksize, cin, eb); }
+
+// kind, operand bytes, N tile, pipeline stages and shared memory of a plan: the weights stay resident next to >= 2 pipeline
+// stages (>= 1 at stride 2).  false when they do not fit.
+static bool tc_tile(const ConvParams& p, int ksize, int stride, TcConvPlan* plan) {
+  const int eb = p.in_dtype == B200ROMP_F32 ? 4 : 2;
+  const int rowb = tc_rowb(ksize, stride, p.cin, eb), kch = p.cin / (rowb / eb);
+  const int budget = 227 * 1024 - 1024 /*align slack*/ - 1024 /*barriers*/;
+  auto bbytes = [&](int n) { return ksize * ksize * kch * n * rowb; };
+  int nt = (p.cout % 64 == 0) ? 64 : 32;
+  int stage_bytes, stages;
+  if (stride == 2) {
+    auto sub_bytes = [&](int i) { return ((i < 2 ? 17 : 16) * ((i & 1) ? 8 : 9) * rowb + 1023) / 1024 * 1024; };
+    stage_bytes = sub_bytes(0) + sub_bytes(1) + sub_bytes(2) + sub_bytes(3);
+    if (nt == 64 && bbytes(64) + 2 * stage_bytes > budget && bbytes(32) + 2 * stage_bytes <= budget) nt = 32;
+    if (nt == 64 && bbytes(64) + stage_bytes > budget) nt = 32;
+    if (bbytes(nt) + stage_bytes > budget) return false;
+    stages = std::min(4, (budget - bbytes(nt)) / stage_bytes);
+  } else {
+    const int hh = 16 + 2 * (ksize / 2), hw = 8 + 2 * (ksize / 2);
+    stage_bytes = (hh * hw * rowb + 1023) / 1024 * 1024;
+    if (bbytes(nt) + 3 * stage_bytes > budget && nt == 64) nt = 32;
+    if (bbytes(nt) + 2 * stage_bytes > budget && nt == 32) nt = 16;   // TF32 3x3 256 -> *: 288 KB of weights at N = 32
+    if (bbytes(nt) + 2 * stage_bytes > budget) return false;
+    stages = std::min((budget - bbytes(nt)) / stage_bytes, 8);   // split into two rings (one per consumer warpgroup)
+  }
+  plan->kind = stride == 2 ? 32 : ksize * 10;
+  plan->eb = eb;
+  plan->cin = p.cin; plan->cout = p.cout; plan->nt = nt;
+  plan->stages = stages;
+  plan->smem_bytes = bbytes(nt) + stages * stage_bytes + 1024 + 1024;
+  return true;
+}
+
+bool tc_conv_supported(const ConvParams& p, int ksize, int stride) {
+  TcConvPlan plan;
+  return tc_shape_supported(p, ksize, stride) && tc_tile(p, ksize, stride, &plan);
 }
 
 template <int MODE, int CIN, int NT, int EB>
@@ -344,107 +383,62 @@ static int dispatch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t st
   return B200ROMP_EINVAL;
 }
 
-static int tc_s2_prepare(const ConvParams& p, const float* w_oihw, int sm_count, TcConvPlan* plan, std::vector<void*>* allocs) {
+int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_oihw, int sm_count, TcConvPlan* plan,
+                    std::vector<void*>* allocs) {
   PFN_encodeTiled encode = tc_get_encode();
   if (!encode) {
     set_error("conv_tc: cuTensorMapEncodeTiled is unavailable");
     return B200ROMP_ECUDA;
   }
-  const int eb = p.in_dtype == B200ROMP_F32 ? 4 : 2;
-  plan->eb = eb;
-  const int rowb = s2_row_bytes(p.cin, eb), cw = rowb / eb, kch = p.cin / cw;
-  auto sub_bytes = [&](int i) { return ((i < 2 ? 17 : 16) * ((i & 1) ? 8 : 9) * rowb + 1023) / 1024 * 1024; };
-  const int stage_bytes = sub_bytes(0) + sub_bytes(1) + sub_bytes(2) + sub_bytes(3);
-  const int budget = 227 * 1024 - 2048;
-  auto bbytes = [&](int n) { return 9 * kch * n * rowb; };
-  int nt = (p.cout % 64 == 0) ? 64 : 32;
-  if (nt == 64 && bbytes(64) + 2 * stage_bytes > budget && bbytes(32) + 2 * stage_bytes <= budget) nt = 32;
-  if (nt == 64 && bbytes(64) + stage_bytes > budget) nt = 32;
-  if (bbytes(nt) + stage_bytes > budget) {
-    set_error("conv_tc: stride-2 cin%d does not fit shared memory", p.cin);
+  if (!tc_tile(p, ksize, stride, plan)) {
+    set_error("conv_tc: k%d s%d cin%d does not fit shared memory", ksize, stride, p.cin);
     return B200ROMP_EINVAL;
   }
-  plan->stages = std::min(4, (budget - bbytes(nt)) / stage_bytes);
-  plan->kind = 32;
-  plan->cin = p.cin; plan->cout = p.cout; plan->nt = nt;
-  plan->grid_y = p.cout / nt;
+  const int eb = plan->eb, rowb = tc_rowb(ksize, stride, p.cin, eb), cw = rowb / eb;
+  plan->grid_y = (p.cout + plan->nt - 1) / plan->nt;
   plan->grid_x = std::max(1, sm_count / plan->grid_y);
-  plan->smem_bytes = bbytes(nt) + plan->stages * stage_bytes + 2048;
-  int rc = tc_pack_weights(w_oihw, p.cin, p.cout, 9, nt, &plan->d_wpack, allocs, rowb, eb);
+  int rc = tc_pack_weights(w_oihw, p.cin, p.cout, ksize * ksize, plan->nt, &plan->d_wpack, allocs, rowb, eb);
   if (rc) return rc;
-  const cuuint64_t C = (cuuint64_t)p.in_C;
-  const cuuint64_t gdim[5] = {2 * C, (cuuint64_t)p.Win / 2, 2, (cuuint64_t)p.Hin / 2, (cuuint64_t)p.B};
-  const cuuint64_t E = (cuuint64_t)eb;
-  const cuuint64_t gstr[4] = {2 * C * E, (cuuint64_t)p.Win * C * E, 2 * (cuuint64_t)p.Win * C * E, (cuuint64_t)p.Hin * p.Win * C * E};
-  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  for (int i = 0; i < 4; ++i) {
-    const cuuint32_t box[5] = {(cuuint32_t)cw, (cuuint32_t)((i & 1) ? 8 : 9), 1, (cuuint32_t)(i < 2 ? 17 : 16), 1};
+  const CUtensorMapDataType dtype = eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const CUtensorMapSwizzle swizzle = rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  if (stride == 2) {
+    // one map per input parity over the space-to-depth view: dims ([pw*C+c], W/2, ph, H/2, N)
+    const cuuint64_t C = (cuuint64_t)p.in_C;
+    const cuuint64_t gdim[5] = {2 * C, (cuuint64_t)p.Win / 2, 2, (cuuint64_t)p.Hin / 2, (cuuint64_t)p.B};
+    const cuuint64_t E = (cuuint64_t)eb;
+    const cuuint64_t gstr[4] = {2 * C * E, (cuuint64_t)p.Win * C * E, 2 * (cuuint64_t)p.Win * C * E, (cuuint64_t)p.Hin * p.Win * C * E};
+    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    for (int i = 0; i < 4; ++i) {
+      const cuuint32_t box[5] = {(cuuint32_t)cw, (cuuint32_t)((i & 1) ? 8 : 9), 1, (cuuint32_t)(i < 2 ? 17 : 16), 1};
+      CUtensorMap tm;
+      CUresult cr = encode(&tm, dtype, 5, const_cast<void*>(p.in), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (cr != CUDA_SUCCESS) {
+        set_error("conv_tc: cuTensorMapEncodeTiled (stride 2) failed with %d", (int)cr);
+        return B200ROMP_ECUDA;
+      }
+      memcpy(plan->tmap_s2[i], &tm, sizeof(tm));
+    }
+  } else {
+    // tensor map over the NHWC input: dims (C slice, W, H, N), halo box, OOB -> zeros
+    const int hh = 16 + 2 * (ksize / 2), hw = 8 + 2 * (ksize / 2);
     CUtensorMap tm;
-    CUresult cr = encode(&tm, eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<void*>(p.in), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+    const cuuint64_t gdim[4] = {(cuuint64_t)p.cin, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
+    const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * eb, (cuuint64_t)p.Win * p.in_C * eb, (cuuint64_t)p.Hin * p.Win * p.in_C * eb};
+    const cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)hw, (cuuint32_t)hh, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * eb);
+    CUresult cr = encode(&tm, dtype, 4, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) {
-      set_error("conv_tc: cuTensorMapEncodeTiled (stride 2) failed with %d", (int)cr);
+      set_error("conv_tc: cuTensorMapEncodeTiled failed with %d", (int)cr);
       return B200ROMP_ECUDA;
     }
-    memcpy(plan->tmap_s2[i], &tm, sizeof(tm));
+    memcpy(plan->tmap_in, &tm, sizeof(tm));
   }
   return dispatch(*plan, p, nullptr, true);
 }
 
-int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_oihw, int sm_count, bool /*ptrs_final*/, TcConvPlan* plan,
-                    std::vector<void*>* allocs) {
-  if (stride == 2) return tc_s2_prepare(p, w_oihw, sm_count, plan, allocs);
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) {
-    set_error("conv_tc: cuTensorMapEncodeTiled is unavailable");
-    return B200ROMP_ECUDA;
-  }
-  const int eb = p.in_dtype == B200ROMP_F32 ? 4 : 2;
-  plan->eb = eb;
-  const int taps = ksize * ksize;
-  const int rowb = tc_row_bytes(ksize, p.cin, eb), cw = rowb / eb, kch = p.cin / cw;
-  // N tile: weights must stay resident next to >= 2 pipeline stages
-  int nt = (p.cout % 64 == 0) ? 64 : 32;
-  const int hh = 16 + 2 * (ksize / 2), hw = 8 + 2 * (ksize / 2);
-  const int stage_bytes = (hh * hw * rowb + 1023) / 1024 * 1024;
-  const int budget = 227 * 1024 - 1024 /*align slack*/ - 1024 /*barriers*/;
-  auto bbytes = [&](int n) { return taps * kch * n * rowb; };
-  if (bbytes(nt) + 3 * stage_bytes > budget && nt == 64) nt = 32;
-  if (bbytes(nt) + 2 * stage_bytes > budget && nt == 32) nt = 16;   // TF32 3x3 256 -> *: 288 KB of weights at N = 32
-  if (bbytes(nt) + 2 * stage_bytes > budget) {
-    set_error("conv_tc: k%d cin%d eb%d does not fit shared memory", ksize, p.cin, eb);
-    return B200ROMP_EINVAL;
-  }
-  plan->stages = std::min((budget - bbytes(nt)) / stage_bytes, 8);   // split into two rings (one per consumer warpgroup)
-  plan->kind = ksize * 10;
-  plan->cin = p.cin; plan->cout = p.cout; plan->nt = nt;
-  plan->grid_y = (p.cout + nt - 1) / nt;
-  plan->grid_x = std::max(1, sm_count / plan->grid_y);
-  plan->smem_bytes = bbytes(nt) + plan->stages * stage_bytes + 1024 + 1024;
-  int rcw = tc_pack_weights(w_oihw, p.cin, p.cout, taps, nt, &plan->d_wpack, allocs, rowb, eb);
-  if (rcw) return rcw;
-  // ---- tensor map over the NHWC input: dims (C slice, W, H, N), halo box, OOB -> zeros
-  CUtensorMap tm;
-  const cuuint64_t gdim[4] = {(cuuint64_t)p.cin, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
-  const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * eb, (cuuint64_t)p.Win * p.in_C * eb, (cuuint64_t)p.Hin * p.Win * p.in_C * eb};
-  const cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)hw, (cuuint32_t)hh, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * eb);
-  CUresult cr = encode(&tm, eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, gdim, gstr, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    set_error("conv_tc: cuTensorMapEncodeTiled failed with %d", (int)cr);
-    return B200ROMP_ECUDA;
-  }
-  memcpy(plan->tmap_in, &tm, sizeof(tm));
-  return dispatch(*plan, p, nullptr, true);
-}
-
-int tc_conv_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) {
-  if (plan.kind == 33) return tc_stem_launch(plan, p, stream);
-  return dispatch(plan, p, stream, false);
-}
+int tc_conv_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) { return dispatch(plan, p, stream, false); }
 
 }  // namespace b200romp

@@ -26,18 +26,18 @@ struct TcConvPlan {
   // bit (tap * 2 + half) = 0 skips the MMAs of that channel half of that tap (all-zero weights of a pixel-pair folded
   // conv, see net.cu fold_pixel_pairs)
   unsigned kmask = 0xFFFFFFFFu;
-  const void* encoded_in = nullptr;   // conv1d engine: input pointer / batch the tensor map was encoded for (external inputs)
+  const void* encoded_in = nullptr;   // conv1d engine: input pointer / batch the tensor map was encoded for
   int encoded_batch = 0;
   void* d_wpack2 = nullptr;           // fused block: conv2's weight image (d_wpack holds conv1's)
   const float* d_bias1 = nullptr;     // fused block: conv1's bias [64] (conv2's is ConvParams::bias)
-  int fold = 0;                       // fused block: runs on the pixel-pair view (both convs folded)
+  int fold = 0;                       // set before prepare: runs on the pixel-pair view (net.cu fold_pixel_pairs)
   std::string describe() const;
 };
 
-// true when (shape, dtypes, flags) can run on the tensor-core engine
-bool tc_conv_supported(const ConvParams& p, int ksize, int stride);
-// packs weights, builds tensor maps, picks the tiling; device allocations are appended to `allocs`
-int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_oihw, int sm_count, bool ptrs_final, TcConvPlan* plan,
+// *_supported: no allocation or CUDA call, a null pointer is a tensor bound later.  A prepare, on a supported shape only,
+// packs weights and builds the plan; device allocations are appended to `allocs`.
+bool tc_conv_supported(const ConvParams& p, int ksize, int stride);   // includes the shared-memory fit of the weights
+int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_oihw, int sm_count, TcConvPlan* plan,
                     std::vector<void*>* allocs);
 int tc_conv_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
 // Conv1d (ksize code 13 = 1x3 along W) engine with streamed weights (conv1d_tc.cu): BEV's bird's-eye-view stack
@@ -46,14 +46,13 @@ int tc_conv1d_prepare(const ConvParams& p, const float* w_oi3, int sm_count, TcC
 int tc_conv1d_launch(TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
 // stem engine (conv_stem_tc.cu): 3->64 3x3 stride-2 conv on raw u8 frames with the input normalisation folded in
 bool tc_stem_supported(const ConvParams& p, int ksize, int stride);
-int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, bool out_final, TcConvPlan* plan,
-                    std::vector<void*>* allocs);
+int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, TcConvPlan* plan, std::vector<void*>* allocs);
 int tc_stem_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
 // fused BasicBlock engine (conv_block_tc.cu): y = relu(conv2(relu(conv1(x) + b1)) + b2 + x), 3x3 stride 1, 64 -> 64 -> 64
 // bf16 NHWC.  `p` describes the block as one op: input and residual x (the same channel slice), output y, bias b2; when
-// `fold` the weights are already the pixel-pair folded ones and `p` the pixel-pair view.
+// plan->fold the weights are already the pixel-pair folded ones and `p` the pixel-pair view.
 bool tc_block_supported(const ConvParams& p);
-int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, bool fold, int sm_count,
+int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
                      TcConvPlan* plan, std::vector<void*>* allocs);
 int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
 

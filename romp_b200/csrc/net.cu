@@ -37,24 +37,28 @@ struct Tensor {
   size_t frame_bytes() const { return (size_t)H * W * C * dtype_size(dtype); }
 };
 
+// The kernel that runs an op.  Sum and MaxPool are set when the op is added, WgmmaBlock by fuse_basic_blocks; every other
+// conv is Simt until choose_kernel decides at finalize.  Generic7x7 and Deconv4x4 are the CUDA-core kernels of
+// resnet_ops.cu; a Wgmma or WgmmaBlock plan with tc.fold runs on the pixel-pair view (fold_pixel_pairs).
+enum class Kernel { Sum, MaxPool, Simt, Generic7x7, Deconv4x4, Wgmma, WgmmaStem, WgmmaConv1d, WgmmaBlock };
+
 struct Op {
-  int kind = 0;                        // 0 = conv (d), 1 = fuse-layer sum (sum; d.out / d.in mirror out / base, d.res = -1)
+  Kernel kernel = Kernel::Simt;
   b200romp_sum_desc sum;
-  b200romp_conv_desc d;
-  std::vector<float> w_host, b_host;   // OIHW fp32, [cout]
-  float* d_w_simt = nullptr;           // [tap][cin][coutPad]
+  b200romp_conv_desc d;                // sum / maxpool: d.out / d.in mirror out / base or in, d.res = -1
+  std::vector<float> w_host, b_host;   // OIHW fp32, [cout]; freed at finalize
+  float* d_w_simt = nullptr;           // CUDA-core kernels only: [tap][cin][coutPad]
   float* d_bias = nullptr;             // [coutPad]
   int coutPad = 0;
-  int engine = B200ROMP_ENGINE_SIMT;   // resolved
-  TcConvPlan tc;                       // tensor-core plan (packed weights, tensor maps)
+  TcConvPlan tc;                       // wgmma kernels: packed weights, tensor maps, tiling
   int lane = 0;                        // concurrency lane inside the captured CUDA graph (b200romp_net_set_lane)
-  int fold = 0;                        // 1 = runs as a pixel-pair folded 64->64 conv on the [H, W/2, 64] view (fold_pixel_pairs)
-  // fused BasicBlock (fuse_basic_blocks): d describes the block (in and res = x, out = y, bias = b2), w_host / b_host are
-  // conv1's, w2_host / b2_host conv2's, `mid` is the intermediate tensor that no longer gets a buffer
-  int block = 0;
+  // WgmmaBlock: d describes the block (in and res = x, out = y, bias = b2), w_host / b_host are conv1's, w2_host / b2_host
+  // conv2's, `mid` is the intermediate tensor that no longer gets a buffer
   int mid = -1;
   std::vector<float> w2_host, b2_host;
 };
+
+static bool on_wgmma(Kernel k) { return k == Kernel::Wgmma || k == Kernel::WgmmaStem || k == Kernel::WgmmaConv1d || k == Kernel::WgmmaBlock; }
 
 }  // namespace b200romp
 
@@ -86,7 +90,9 @@ struct b200romp_net {
   bool use_lanes = false;
 };
 
-static int fill_params(b200romp_net* net, const Op& op, int batch, ConvParams* out) {
+// `allow_unbound` (planning): a tensor without storage yet - internal before buffer planning, external before
+// b200romp_net_bind - leaves a null pointer.  Launches require every pointer.
+static int fill_params(const b200romp_net* net, const Op& op, int batch, bool allow_unbound, ConvParams* out) {
   const b200romp_conv_desc& d = op.d;
   const Tensor& ti = net->tensors[d.in];
   const Tensor& to = net->tensors[d.out];
@@ -106,11 +112,11 @@ static int fill_params(b200romp_net* net, const Op& op, int batch, ConvParams* o
   }
   p.relu = d.relu; p.pow_channel = d.pow_channel; p.out_nchw = to.nchw;
   p.in_dtype = ti.dtype; p.out_dtype = to.dtype; p.input_norm = d.input_norm;
-  if (op.fold) {   // the same bytes seen as [B, H, W/2, 2C]: two horizontally adjacent pixels form one 64-channel pixel
+  if (op.tc.fold) {   // the same bytes seen as [B, H, W/2, 2C]: two horizontally adjacent pixels form one 64-channel pixel
     p.Win /= 2; p.Wout /= 2;
     p.in_C *= 2; p.cin *= 2; p.out_C *= 2; p.cout *= 2; p.res_C *= 2;
   }
-  if (!p.in || !p.out) {
+  if (!allow_unbound && (!p.in || !p.out)) {
     set_error("op uses an unbound tensor (in=%d out=%d)", d.in, d.out);
     return B200ROMP_ESTATE;
   }
@@ -248,7 +254,7 @@ int b200romp_net_add_sum(b200romp_net* net, const b200romp_sum_desc* desc) {
                 "add_sum: term %d is %dx%dx%d (slice from channel %d), expected %dx%dx%d", k, tt.H, tt.W, tt.C, co, to.H / u, to.W / u, to.C);
   }
   Op op;
-  op.kind = 1;
+  op.kernel = Kernel::Sum;
   op.sum = *desc;
   memset(&op.d, 0, sizeof(op.d));
   op.d.out = desc->out; op.d.in = desc->base; op.d.res = -1;
@@ -265,7 +271,7 @@ int b200romp_net_add_maxpool(b200romp_net* net, int in, int out) {
   B2R_REQUIRE(!ti.nchw && !to.nchw && ti.dtype == to.dtype && ti.dtype != B200ROMP_U8 && ti.C == to.C, "add_maxpool: NHWC bf16/fp32 tensors of equal C");
   B2R_REQUIRE(to.H == (ti.H + 2 - 3) / 2 + 1 && to.W == (ti.W + 2 - 3) / 2 + 1, "add_maxpool: output must be %dx%d", (ti.H - 1) / 2 + 1, (ti.W - 1) / 2 + 1);
   Op op;
-  op.kind = 2;
+  op.kernel = Kernel::MaxPool;
   memset(&op.d, 0, sizeof(op.d));
   memset(&op.sum, 0, sizeof(op.sum));
   op.d.in = in; op.d.out = out; op.d.res = -1;
@@ -294,45 +300,38 @@ static int fill_sum_params(b200romp_net* net, const Op& op, int batch, SumParams
 
 // one op of the plan on `stream`
 static int enqueue_op(b200romp_net* net, Op& op, int batch, cudaStream_t stream) {
-  if (op.kind == 1) {
-    SumParams sp;
-    int rc = fill_sum_params(net, op, batch, &sp);
-    return rc ? rc : launch_fuse_sum(sp, stream);
-  }
-  if (op.kind == 2) {
-    const Tensor& ti = net->tensors[op.d.in];
-    const Tensor& to = net->tensors[op.d.out];
-    B2R_REQUIRE(ti.ptr && to.ptr, "maxpool op: unbound tensor");
-    return launch_maxpool3x3s2(ti.ptr, to.ptr, ti.dtype, batch, ti.H, ti.W, ti.C, stream);
-  }
   ConvParams p;
-  int rc = fill_params(net, op, batch, &p);
-  if (rc) return rc;
-  if (op.block) return tc_block_launch(op.tc, p, stream);
-  if (op.d.ksize == 7) return launch_conv_generic(p, 7, op.d.stride, stream);
-  if (op.d.ksize == 42) return launch_deconv4x4s2(p, stream);
-  if (op.engine == B200ROMP_ENGINE_TCGEN05) return op.tc.kind == 13 ? tc_conv1d_launch(op.tc, p, stream) : tc_conv_launch(op.tc, p, stream);
-  return launch_conv_simt(p, op.d.ksize, op.d.stride, stream);
+  if (op.kernel != Kernel::Sum && op.kernel != Kernel::MaxPool) {
+    int rc = fill_params(net, op, batch, false, &p);
+    if (rc) return rc;
+  }
+  switch (op.kernel) {
+    case Kernel::Sum: {
+      SumParams sp;
+      int rc = fill_sum_params(net, op, batch, &sp);
+      return rc ? rc : launch_fuse_sum(sp, stream);
+    }
+    case Kernel::MaxPool: {
+      const Tensor& ti = net->tensors[op.d.in];
+      const Tensor& to = net->tensors[op.d.out];
+      B2R_REQUIRE(ti.ptr && to.ptr, "maxpool op: unbound tensor");
+      return launch_maxpool3x3s2(ti.ptr, to.ptr, ti.dtype, batch, ti.H, ti.W, ti.C, stream);
+    }
+    case Kernel::Simt: return launch_conv_simt(p, op.d.ksize, op.d.stride, stream);
+    case Kernel::Generic7x7: return launch_conv_generic(p, 7, op.d.stride, stream);
+    case Kernel::Deconv4x4: return launch_deconv4x4s2(p, stream);
+    case Kernel::Wgmma: return tc_conv_launch(op.tc, p, stream);
+    case Kernel::WgmmaStem: return tc_stem_launch(op.tc, p, stream);
+    case Kernel::WgmmaConv1d: return tc_conv1d_launch(op.tc, p, stream);
+    case Kernel::WgmmaBlock: return tc_block_launch(op.tc, p, stream);
+  }
+  return B200ROMP_EINVAL;
 }
 
-static int upload_simt_weights(b200romp_net* net, Op& op) {
-  const b200romp_conv_desc& d = op.d;
-  const int taps = conv_taps(d.ksize);
-  op.coutPad = (d.cout + 63) / 64 * 64;
-  std::vector<float> packed((size_t)taps * d.cin * op.coutPad, 0.f);
-  for (int co = 0; co < d.cout; ++co)
-    for (int ci = 0; ci < d.cin; ++ci)
-      for (int t = 0; t < taps; ++t)   // conv: OIHW; ConvTranspose2d (code 42): PyTorch's [cin][cout][4][4]
-        packed[((size_t)t * d.cin + ci) * op.coutPad + co] =
-            d.ksize == 42 ? op.w_host[((size_t)ci * d.cout + co) * taps + t] : op.w_host[((size_t)co * d.cin + ci) * taps + t];
-  std::vector<float> bias(op.coutPad, 0.f);
-  std::copy(op.b_host.begin(), op.b_host.end(), bias.begin());
-  B2R_CUDA_OK(cudaMalloc(&op.d_w_simt, packed.size() * sizeof(float)));
-  net->device_allocs.push_back(op.d_w_simt);
-  B2R_CUDA_OK(cudaMemcpy(op.d_w_simt, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
-  B2R_CUDA_OK(cudaMalloc(&op.d_bias, bias.size() * sizeof(float)));
-  net->device_allocs.push_back(op.d_bias);
-  B2R_CUDA_OK(cudaMemcpy(op.d_bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
+static int upload(b200romp_net* net, const std::vector<float>& v, float** d) {
+  B2R_CUDA_OK(cudaMalloc(d, v.size() * sizeof(float)));
+  net->device_allocs.push_back(*d);
+  B2R_CUDA_OK(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
   return B200ROMP_OK;
 }
 
@@ -359,9 +358,9 @@ static bool fold_eligible(const b200romp_net* net, const Op& op) {
   return true;
 }
 
-static void fold_pixel_pairs(const std::vector<float>& w, const std::vector<float>& b, std::vector<float>* w2, std::vector<float>* b2,
-                             unsigned* kmask) {
-  w2->assign((size_t)64 * 64 * 9, 0.f);
+// in place: [32][32][3][3] weights and [32] bias -> the [64][64][3][3] pair-view weights and [64] bias
+static void fold_pixel_pairs(std::vector<float>* w, std::vector<float>* b) {
+  std::vector<float> w2((size_t)64 * 64 * 9, 0.f), b2(64);
   for (int dx = 0; dx < 2; ++dx)
     for (int co = 0; co < 32; ++co)
       for (int h = 0; h < 2; ++h)
@@ -370,29 +369,35 @@ static void fold_pixel_pairs(const std::vector<float>& w, const std::vector<floa
             for (int s = -1; s <= 1; ++s) {
               const int kx = 2 * s + h - dx + 1;
               if (kx < 0 || kx > 2) continue;
-              (*w2)[(((size_t)(dx * 32 + co) * 64 + h * 32 + ci) * 3 + ky) * 3 + (s + 1)] = w[(((size_t)co * 32 + ci) * 3 + ky) * 3 + kx];
+              w2[(((size_t)(dx * 32 + co) * 64 + h * 32 + ci) * 3 + ky) * 3 + (s + 1)] = (*w)[(((size_t)co * 32 + ci) * 3 + ky) * 3 + kx];
             }
-  b2->assign(64, 0.f);
-  for (int i = 0; i < 64; ++i) (*b2)[i] = (i % 32) < (int)b.size() ? b[i % 32] : 0.f;
+  for (int i = 0; i < 64; ++i) b2[i] = (*b)[i % 32];
+  *w = std::move(w2);
+  *b = std::move(b2);
+}
+
+// TcConvPlan::kmask of a folded conv
+static unsigned fold_kmask() {
   unsigned m = 0;
   for (int t = 0; t < 9; ++t) {
     const int s = t % 3 - 1;
     if (s != -1) m |= 1u << (t * 2 + 0);   // first pixel of the pair is used by s = 0, +1
     if (s != +1) m |= 1u << (t * 2 + 1);   // second pixel by s = -1, 0
   }
-  *kmask = m;
+  return m;
 }
 
 // HRNet BasicBlocks relu(conv2(relu(conv1(x))) + x) whose convs are 3x3 stride-1 64->64 (or pixel-pair foldable 32->32) bf16
 // layers become one op on the fused block kernel (conv_block_tc.cu): the intermediate never reaches HBM and x is read once.
-// Ops i, i+1 fuse when conv2 reads exactly conv1's output, that tensor is internal and read by nothing else, and conv2's
-// residual is conv1's input slice.  A caller that binds the intermediate as an external tensor keeps the two convs.
+// Ops i, i+1 fuse when conv2 reads exactly conv1's output, that tensor is internal and read by nothing else, conv2's
+// residual is conv1's input slice, and the block kernel supports the fused op.  A caller that binds the intermediate as an
+// external tensor keeps the two convs.
 static bool is_bf16_block_conv(const b200romp_net* net, const Op& op) {
   const b200romp_conv_desc& d = op.d;
   const Tensor& ti = net->tensors[d.in];
   const Tensor& to = net->tensors[d.out];
-  return op.kind == 0 && d.ksize == 3 && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
-         (d.engine == B200ROMP_ENGINE_AUTO || d.engine == B200ROMP_ENGINE_TCGEN05) && ti.dtype == B200ROMP_BF16 &&
+  return d.ksize == 3 && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
+         (d.engine == B200ROMP_ENGINE_AUTO || d.engine == B200ROMP_ENGINE_WGMMA) && ti.dtype == B200ROMP_BF16 &&
          to.dtype == B200ROMP_BF16 && !to.nchw && d.cin == d.cout && (d.cin == 64 || d.cin == 32);
 }
 
@@ -402,7 +407,7 @@ static void fuse_basic_blocks(b200romp_net* net) {
   for (const Op& op : net->ops) {
     ++reads[op.d.in];
     ++writes[op.d.out];
-    if (op.kind == 1)
+    if (op.kernel == Kernel::Sum)
       for (int k = 0; k < op.sum.n_terms; ++k) ++reads[op.sum.term[k]];
     else if (op.d.res >= 0) ++reads[op.d.res];
   }
@@ -413,40 +418,35 @@ static void fuse_basic_blocks(b200romp_net* net) {
     if (i + 1 < net->ops.size()) {
       Op& b = net->ops[i + 1];
       const int x = a.d.in, t = a.d.out;
-      const Tensor& tx = net->tensors[x];
       const Tensor& tt = net->tensors[t];
       const int C = a.d.cin;
       bool ok = is_bf16_block_conv(net, a) && is_bf16_block_conv(net, b) && a.d.res < 0 && b.d.cin == C && a.lane == b.lane &&
                 b.d.in == t && b.d.in_c_off == 0 && a.d.out_c_off == 0 && tt.C == C && !tt.external && !tt.constant &&
                 reads[t] == 1 && writes[t] == 1 && b.d.res == x && b.d.res_c_off == a.d.in_c_off && !b.d.res_broadcast &&
-                !tx.external && tx.H % 16 == 0;
-      bool fold = false;
-      if (ok && C == 32) {
-        fold = fold_eligible(net, a) && fold_eligible(net, b);   // the 32-channel kernel is the folded 64-channel one
-        ok = fold;
-      }
-      if (ok && C == 64) {
-        const Tensor& ty = net->tensors[b.d.out];
-        ok = !ty.external && tx.W % 8 == 0 && tx.C % 8 == 0 && a.d.in_c_off % 8 == 0 && ty.C % 8 == 0 && b.d.out_c_off % 8 == 0;
-      }
+                !net->tensors[x].external && !net->tensors[b.d.out].external &&
+                (C == 64 || (fold_eligible(net, a) && fold_eligible(net, b)));   // the 32-channel kernel is the folded 64-channel one
       if (ok) {
         Op f;
+        f.kernel = Kernel::WgmmaBlock;
         f.d = a.d;
         f.d.out = b.d.out;
         f.d.out_c_off = b.d.out_c_off;
         f.d.res = x;
         f.d.res_c_off = b.d.res_c_off;
-        f.block = 1;
-        f.fold = fold ? 1 : 0;
-        f.mid = t;
-        f.lane = a.lane;
-        f.w_host = std::move(a.w_host);
-        f.b_host = std::move(a.b_host);
-        f.w2_host = std::move(b.w_host);
-        f.b2_host = std::move(b.b_host);
-        fused.push_back(std::move(f));
-        ++i;
-        continue;
+        f.tc.fold = C == 32;
+        ConvParams p;
+        fill_params(net, f, 1, true, &p);
+        if (tc_block_supported(p)) {
+          f.mid = t;
+          f.lane = a.lane;
+          f.w_host = std::move(a.w_host);
+          f.b_host = std::move(a.b_host);
+          f.w2_host = std::move(b.w_host);
+          f.b2_host = std::move(b.b_host);
+          fused.push_back(std::move(f));
+          ++i;
+          continue;
+        }
       }
     }
     fused.push_back(std::move(a));
@@ -454,27 +454,79 @@ static void fuse_basic_blocks(b200romp_net* net) {
   net->ops = std::move(fused);
 }
 
-// weights, biases and plan of a fused block op (the engine resolution of fuse_basic_blocks' ops)
-static int prepare_block(b200romp_net* net, Op& op, int max_batch) {
-  std::vector<float> w1 = op.w_host, b1 = op.b_host, w2 = op.w2_host, b2 = op.b2_host;
-  if (op.fold) {
-    unsigned kmask = 0;
-    fold_pixel_pairs(op.w_host, op.b_host, &w1, &b1, &kmask);
-    fold_pixel_pairs(op.w2_host, op.b2_host, &w2, &b2, &kmask);
+// Decides op.kernel (and op.tc.fold) of a conv from its descriptor, the requested engine and its tensors' shapes, dtypes and
+// flags.  No allocation, no CUDA call: a shape the wgmma engines cannot take runs on the SIMT engine unless the descriptor
+// forces B200ROMP_ENGINE_WGMMA.
+static int choose_kernel(const b200romp_net* net, int i, Op& op) {
+  const b200romp_conv_desc& d = op.d;
+  const Tensor& ti = net->tensors[d.in];
+  const Tensor& to = net->tensors[d.out];
+  if (d.ksize == 7 || d.ksize == 42) {
+    op.kernel = d.ksize == 7 ? Kernel::Generic7x7 : Kernel::Deconv4x4;
+    return B200ROMP_OK;
   }
-  op.coutPad = 64;
-  B2R_CUDA_OK(cudaMalloc(&op.d_bias, 64 * sizeof(float)));
-  net->device_allocs.push_back(op.d_bias);
-  B2R_CUDA_OK(cudaMemcpy(op.d_bias, b2.data(), 64 * sizeof(float), cudaMemcpyHostToDevice));
+  op.kernel = Kernel::Simt;
+  const bool forced = d.engine == B200ROMP_ENGINE_WGMMA;
+  const bool stem = ti.dtype == B200ROMP_U8 && d.cin == 3 && d.ksize == 3 && d.stride == 2;
+  if (!forced && !(d.engine == B200ROMP_ENGINE_TF32 && ti.dtype == B200ROMP_F32) &&
+      !(d.engine == B200ROMP_ENGINE_AUTO && (ti.dtype == B200ROMP_BF16 || stem)))
+    return B200ROMP_OK;
   ConvParams p;
-  int rc = fill_params(net, op, max_batch, &p);
-  if (rc) return rc;
-  rc = tc_block_prepare(p, w1.data(), b1.data(), w2.data(), op.fold != 0, net->sm_count, &op.tc, &net->device_allocs);
-  if (rc) return rc;
-  op.engine = B200ROMP_ENGINE_TCGEN05;
-  op.w_host.clear(); op.w_host.shrink_to_fit();
-  op.w2_host.clear(); op.w2_host.shrink_to_fit();
+  fill_params(net, op, net->max_batch, true, &p);
+  if (stem) {
+    // the stem gathers its u8 input with plain loads (it may be external); its output must be internal
+    if (!to.external && d.res < 0 && tc_stem_supported(p, d.ksize, d.stride)) op.kernel = Kernel::WgmmaStem;
+  } else if (d.ksize == 13) {
+    if (tc_conv1d_supported(p)) op.kernel = Kernel::WgmmaConv1d;   // input tensor map encoded at launch: may be external
+  } else if (!ti.external && tc_conv_supported(p, d.ksize, d.stride)) {   // input tensor map encoded at finalize
+    op.kernel = Kernel::Wgmma;
+    op.tc.fold = fold_eligible(net, op);
+  }
+  if (forced && op.kernel == Kernel::Simt) {
+    set_error("op %d: tensor-core engine forced but shape unsupported", i);
+    return B200ROMP_EINVAL;
+  }
   return B200ROMP_OK;
+}
+
+// Uploads what op's kernel reads and builds its plan.  Every conv gets its bias zero-padded to a multiple of 64 (the wgmma
+// epilogues read up to grid_y * NT); only the CUDA-core kernels get the [tap][cin][coutPad] fp32 weights.
+static int prepare_op(b200romp_net* net, Op& op) {
+  if (op.kernel == Kernel::Sum || op.kernel == Kernel::MaxPool) return B200ROMP_OK;
+  const b200romp_conv_desc& d = op.d;
+  std::vector<float> w = std::move(op.w_host), b = std::move(op.b_host), w2 = std::move(op.w2_host), b2 = std::move(op.b2_host);
+  if (op.tc.fold) {
+    fold_pixel_pairs(&w, &b);
+    if (op.kernel == Kernel::WgmmaBlock) fold_pixel_pairs(&w2, &b2);
+  }
+  std::vector<float> bias = op.kernel == Kernel::WgmmaBlock ? b2 : b;   // a block's bias is conv2's
+  op.coutPad = ((int)bias.size() + 63) / 64 * 64;
+  bias.resize(op.coutPad, 0.f);
+  int rc = upload(net, bias, &op.d_bias);
+  if (rc) return rc;
+  ConvParams p;
+  fill_params(net, op, net->max_batch, true, &p);
+  switch (op.kernel) {
+    case Kernel::Simt:
+    case Kernel::Generic7x7:
+    case Kernel::Deconv4x4: {
+      const int taps = conv_taps(d.ksize);
+      std::vector<float> packed((size_t)taps * d.cin * op.coutPad, 0.f);
+      for (int co = 0; co < d.cout; ++co)
+        for (int ci = 0; ci < d.cin; ++ci)
+          for (int t = 0; t < taps; ++t)   // conv: OIHW; ConvTranspose2d (code 42): PyTorch's [cin][cout][4][4]
+            packed[((size_t)t * d.cin + ci) * op.coutPad + co] =
+                d.ksize == 42 ? w[((size_t)ci * d.cout + co) * taps + t] : w[((size_t)co * d.cin + ci) * taps + t];
+      return upload(net, packed, &op.d_w_simt);
+    }
+    case Kernel::Wgmma:
+      if (op.tc.fold) op.tc.kmask = fold_kmask();
+      return tc_conv_prepare(p, d.ksize, d.stride, w.data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaStem: return tc_stem_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaConv1d: return tc_conv1d_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaBlock: return tc_block_prepare(p, w.data(), b.data(), w2.data(), net->sm_count, &op.tc, &net->device_allocs);
+    default: return B200ROMP_OK;
+  }
 }
 
 int b200romp_net_finalize(b200romp_net* net, int max_batch) {
@@ -490,7 +542,7 @@ int b200romp_net_finalize(b200romp_net* net, int max_batch) {
     to.last_use = std::max(to.last_use, i);
     net->tensors[d.in].last_use = std::max(net->tensors[d.in].last_use, i);
     if (d.res >= 0) net->tensors[d.res].last_use = std::max(net->tensors[d.res].last_use, i);
-    if (net->ops[i].kind == 1)
+    if (net->ops[i].kernel == Kernel::Sum)
       for (int k = 0; k < net->ops[i].sum.n_terms; ++k) {
         Tensor& tt = net->tensors[net->ops[i].sum.term[k]];
         B2R_REQUIRE(tt.external || tt.constant || (tt.first_def >= 0 && tt.first_def < i), "op %d sums tensor %d before it is written", i, net->ops[i].sum.term[k]);
@@ -542,83 +594,12 @@ int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   for (int t = 0; t < nT; ++t)
     if (tensor_buf[t] >= 0) net->tensors[t].ptr = net->workspace + bufs[tensor_buf[t]].offset;
   net->max_batch = max_batch;
-  // ---- engine resolution + weight upload
+  // ---- kernel choice, weight upload, plans
   for (int i = 0; i < nO; ++i) {
     Op& op = net->ops[i];
-    if (op.kind == 1 || op.kind == 2) continue;
-    if (op.block) {
-      int rc = prepare_block(net, op, max_batch);
-      if (rc) return rc;
-      continue;
-    }
-    int rc = upload_simt_weights(net, op);
+    int rc = op.kernel == Kernel::Simt ? choose_kernel(net, i, op) : B200ROMP_OK;   // Simt: a conv as added
+    if (!rc) rc = prepare_op(net, op);
     if (rc) return rc;
-    op.engine = B200ROMP_ENGINE_SIMT;
-    const Tensor& ti = net->tensors[op.d.in];
-    const Tensor& to = net->tensors[op.d.out];
-    const bool stem_like = ti.dtype == B200ROMP_U8 && op.d.cin == 3 && op.d.ksize == 3 && op.d.stride == 2;
-    if (op.d.ksize == 7 || op.d.ksize == 42) { op.w_host.clear(); op.w_host.shrink_to_fit(); continue; }   // CUDA-core kernels of resnet_ops.cu
-    const bool want_tf32 = op.d.engine == B200ROMP_ENGINE_TF32 && ti.dtype == B200ROMP_F32;
-    const bool want_tc = op.d.engine == B200ROMP_ENGINE_TCGEN05 || want_tf32 ||
-                         (op.d.engine == B200ROMP_ENGINE_AUTO && (ti.dtype == B200ROMP_BF16 || stem_like));
-    if (want_tc) {
-      ConvParams p;
-      // The TMA tensor map of the INPUT is baked now, so the input must be an internal tensor (final pointer);
-      // outputs / residuals are plain pointers read from ConvParams at launch and may be external (map outputs).
-      // (The stem engine gathers its u8 input with plain loads: its input may be external, its output must be internal.)
-      bool ext_out_unbound = false, ext_in_unbound = false;
-      if (to.external && to.ptr == nullptr) {   // give fill_params a placeholder; the real pointer comes at run time
-        net->tensors[op.d.out].ptr = reinterpret_cast<void*>(16);
-        ext_out_unbound = true;
-      }
-      const bool conv1d = op.d.ksize == 13;
-      if ((stem_like || conv1d) && ti.external && ti.ptr == nullptr) {
-        net->tensors[op.d.in].ptr = reinterpret_cast<void*>(16);
-        ext_in_unbound = true;
-      }
-      const bool params_ok = (!ti.external || stem_like || conv1d) && fill_params(net, op, max_batch, &p) == B200ROMP_OK;
-      if (ext_out_unbound) net->tensors[op.d.out].ptr = nullptr;
-      if (ext_in_unbound) net->tensors[op.d.in].ptr = nullptr;
-      const bool ptrs_final = !to.external && (op.d.res < 0 || !net->tensors[op.d.res].external);
-      if (params_ok && stem_like && ptrs_final && tc_stem_supported(p, op.d.ksize, op.d.stride)) {
-        rc = tc_stem_prepare(p, op.w_host.data(), net->sm_count, ptrs_final, &op.tc, &net->device_allocs);
-        if (rc == B200ROMP_OK) op.engine = B200ROMP_ENGINE_TCGEN05;
-        else if (op.d.engine == B200ROMP_ENGINE_TCGEN05) return rc;
-      } else if (params_ok && conv1d && ti.dtype == B200ROMP_BF16 && tc_conv1d_supported(p)) {
-        // (an external input only has a placeholder pointer here: the tensor map is re-encoded at launch)
-        rc = tc_conv1d_prepare(p, op.w_host.data(), net->sm_count, &op.tc, &net->device_allocs);
-        if (rc == B200ROMP_OK) op.engine = B200ROMP_ENGINE_TCGEN05;
-        else if (op.d.engine == B200ROMP_ENGINE_TCGEN05) return rc;
-      } else if (params_ok && !stem_like && !conv1d && (ti.dtype != B200ROMP_F32 || want_tf32 || op.d.engine == B200ROMP_ENGINE_TCGEN05) &&
-                 tc_conv_supported(p, op.d.ksize, op.d.stride)) {
-        rc = -1;
-        if (fold_eligible(net, op)) {
-          std::vector<float> w2, b2;
-          unsigned kmask = 0;
-          fold_pixel_pairs(op.w_host, op.b_host, &w2, &b2, &kmask);
-          ConvParams pf;
-          op.fold = 1;
-          TcConvPlan plan;
-          if (fill_params(net, op, max_batch, &pf) == B200ROMP_OK && tc_conv_supported(pf, 3, 1) &&
-              tc_conv_prepare(pf, 3, 1, w2.data(), net->sm_count, ptrs_final, &plan, &net->device_allocs) == B200ROMP_OK && plan.kind == 30 && plan.nt == 64) {
-            plan.kmask = kmask;
-            op.tc = plan;
-            B2R_CUDA_OK(cudaMemcpy(op.d_bias, b2.data(), 64 * sizeof(float), cudaMemcpyHostToDevice));   // coutPad = 64
-            rc = B200ROMP_OK;
-          } else {
-            op.fold = 0;
-          }
-        }
-        if (rc != B200ROMP_OK)
-          rc = tc_conv_prepare(p, op.d.ksize, op.d.stride, op.w_host.data(), net->sm_count, ptrs_final, &op.tc, &net->device_allocs);
-        if (rc == B200ROMP_OK) op.engine = B200ROMP_ENGINE_TCGEN05;
-        else if (op.d.engine == B200ROMP_ENGINE_TCGEN05) return rc;
-      } else if (op.d.engine == B200ROMP_ENGINE_TCGEN05) {
-        set_error("op %d: tensor-core engine forced but shape unsupported", i);
-        return B200ROMP_EINVAL;
-      }
-    }
-    op.w_host.clear(); op.w_host.shrink_to_fit();
   }
   net->finalized = true;
   return B200ROMP_OK;
@@ -665,7 +646,7 @@ static int enqueue_all_lanes(b200romp_net* net, int batch, cudaStream_t stream) 
     const void* write = net->tensors[op.d.out].ptr;
     auto add_read = [&](int t) { if (t >= 0 && !net->tensors[t].constant) reads.push_back(net->tensors[t].ptr); };
     add_read(op.d.in);
-    if (op.kind == 1) for (int k = 0; k < op.sum.n_terms; ++k) add_read(op.sum.term[k]);
+    if (op.kernel == Kernel::Sum) for (int k = 0; k < op.sum.n_terms; ++k) add_read(op.sum.term[k]);
     else add_read(op.d.res);
     std::vector<int> deps;
     for (const void* r : reads) { auto it = acc.find(r); if (it != acc.end() && it->second.writer >= 0) deps.push_back(it->second.writer); }
@@ -796,32 +777,30 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
     const b200romp_conv_desc& d = op.d;
     const Tensor& ti = net->tensors[d.in];
     const Tensor& to = net->tensors[d.out];
-    if (op.kind == 2) {
-      snprintf(line, sizeof(line), "op%03zu maxpool 3x3 s2 in t%d[%dx%dx%d] out t%d[%dx%dx%d]\n", i, d.in, ti.H, ti.W, ti.C, d.out, to.H, to.W, to.C);
-      s += line;
-      continue;
+    switch (op.kernel) {
+      case Kernel::MaxPool:
+        snprintf(line, sizeof(line), "op%03zu maxpool 3x3 s2 in t%d[%dx%dx%d] out t%d[%dx%dx%d]\n", i, d.in, ti.H, ti.W, ti.C, d.out, to.H, to.W, to.C);
+        break;
+      case Kernel::Sum: {
+        int n = snprintf(line, sizeof(line), "op%03zu sum     out t%d[%dx%dx%d] = relu%d( t%d", i, op.sum.out, to.H, to.W, to.C, op.sum.relu, op.sum.base);
+        for (int k = 0; k < op.sum.n_terms; ++k) n += snprintf(line + n, sizeof(line) - n, " + up%d(t%d)", op.sum.up[k], op.sum.term[k]);
+        snprintf(line + n, sizeof(line) - n, " )\n");
+        break;
+      }
+      case Kernel::WgmmaBlock: {   // one launch, two convs: a folded block runs both of them on pixel pairs
+        const Tensor& tm = net->tensors[op.mid];
+        snprintf(line, sizeof(line),
+                 "op%03zu wgmma   block k3 s1 %d->%d->%d in t%d[%dx%dx%d]+%d mid t%d[%dx%dx%d] out t%d[%dx%dx%d]+%d res t%d+%d up1 relu1 "
+                 "bias1 bias2 [tc-block grid %d smem %d%s]\n",
+                 i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
+                 d.out_c_off, d.res, d.res_c_off, op.tc.grid_x, op.tc.smem_bytes, op.tc.fold ? " conv1 pixel-pairs conv2 pixel-pairs" : "");
+        break;
+      }
+      default:
+        snprintf(line, sizeof(line), "op%03zu %s k%d s%d %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up%d relu%d%s\n", i,
+                 on_wgmma(op.kernel) ? "wgmma  " : "simt   ", d.ksize, d.stride, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, d.out,
+                 to.H, to.W, to.C, d.out_c_off, d.res, d.upsample, d.relu, on_wgmma(op.kernel) ? op.tc.describe().c_str() : "");
     }
-    if (op.kind == 1) {
-      int n = snprintf(line, sizeof(line), "op%03zu sum     out t%d[%dx%dx%d] = relu%d( t%d", i, op.sum.out, to.H, to.W, to.C, op.sum.relu, op.sum.base);
-      for (int k = 0; k < op.sum.n_terms; ++k) n += snprintf(line + n, sizeof(line) - n, " + up%d(t%d)", op.sum.up[k], op.sum.term[k]);
-      snprintf(line + n, sizeof(line) - n, " )\n");
-      s += line;
-      continue;
-    }
-    if (op.block) {   // one launch, two convs: a folded block runs both of them on pixel pairs
-      const Tensor& tm = net->tensors[op.mid];
-      snprintf(line, sizeof(line),
-               "op%03zu wgmma   block k3 s1 %d->%d->%d in t%d[%dx%dx%d]+%d mid t%d[%dx%dx%d] out t%d[%dx%dx%d]+%d res t%d+%d up1 relu1 "
-               "bias1 bias2 [tc-block grid %d smem %d%s]\n",
-               i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
-               d.out_c_off, d.res, d.res_c_off, op.tc.grid_x, op.tc.smem_bytes, op.fold ? " conv1 pixel-pairs conv2 pixel-pairs" : "");
-      s += line;
-      continue;
-    }
-    snprintf(line, sizeof(line), "op%03zu %s k%d s%d %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up%d relu%d%s\n", i,
-             op.engine == B200ROMP_ENGINE_TCGEN05 ? "wgmma  " : "simt   ", d.ksize, d.stride, d.cin, d.cout, d.in, ti.H,
-             ti.W, ti.C, d.in_c_off, d.out, to.H, to.W, to.C, d.out_c_off, d.res, d.upsample, d.relu,
-             op.engine == B200ROMP_ENGINE_TCGEN05 ? op.tc.describe().c_str() : "");
     s += line;
   }
   snprintf(line, sizeof(line), "workspace %.1f MiB for max_batch %d\n", net->workspace_bytes / 1048576.0, net->max_batch);

@@ -39,7 +39,7 @@ def test_epilogue_writes_only_its_channel_slice(case):
     res = torch.randn(B, Ho, Wo, out_C, generator=g).to(td).cuda()
     sentinel = 1024.0   # exact in bf16
     out = torch.full((B, Ho, Wo, out_C), sentinel, dtype=td, device="cuda")
-    engine = _lib.ENGINE_TCGEN05 if dt == BF16 else _lib.ENGINE_TF32
+    engine = _lib.ENGINE_WGMMA if dt == BF16 else _lib.ENGINE_TF32
     d = ConvDesc(0, 0, 0, off, -1, off, bcast, cin, cout, k, stride, 1, 1, 0, -1, engine)
     lib = _lib.load()
     rc = lib.b200romp_conv2d(C.byref(d), np.ascontiguousarray(w, np.float32).ctypes.data_as(C.POINTER(C.c_float)),

@@ -1,5 +1,5 @@
 """wgmma conv engine (csrc/conv_tc.cu, conv_stem_tc.cu) through the C ABI (b200romp_conv2d, engine forced
-to TCGEN05) against a plain fp32 torch conv on the same bf16-rounded operands.  Covers every kernel family / epilogue:
+to WGMMA) against a plain fp32 torch conv on the same bf16-rounded operands.  Covers every kernel family / epilogue:
 1x1, 3x3 stride 1 (halo tile + shifted descriptors), 3x3 stride 2 (space-to-depth maps), direct epilogue (fp32 out,
 fp32 residual, upsampled output, NCHW maps), bf16 out and bf16 residual,
 multi-tile persistent loops, and the u8 stem.  Tolerance: fp32 accumulation of bf16 products - only the summation
@@ -55,7 +55,7 @@ def test_tcgen05_conv_matches_torch(case):
         if res_mode == 2:
             res = res.bfloat16()
     got = conv2d(x, w, b, stride=stride, relu=bool(relu), res=res, up=up, out_dtype=BF16 if out_bf16 else F32,
-                 engine=_lib.ENGINE_TCGEN05).float().cpu()
+                 engine=_lib.ENGINE_WGMMA).float().cpu()
     ref = conv_ref(x, w, b, stride=stride, relu=bool(relu), res=res, up=up)
     tol = 2e-4 + (2.0 ** -8) * ref.abs() if out_bf16 else 2e-4 + 1e-5 * ref.abs()
     bad = (got - ref).abs() > tol
@@ -68,7 +68,7 @@ def test_tcgen05_nchw_map_output_with_pow():
     x = torch.from_numpy(rs.normal(0, 1, (2, 32, 32, 64)).astype(np.float32)).cuda().bfloat16()
     w = torch.from_numpy(rs.normal(0, 0.125, (35, 64, 1, 1)).astype(np.float32)).bfloat16().float().numpy()
     b = rs.normal(0, 0.5, 35).astype(np.float32)
-    got = conv2d(x, w, b, out_dtype=F32, engine=_lib.ENGINE_TCGEN05, out_nchw=1, pow_channel=0).cpu()
+    got = conv2d(x, w, b, out_dtype=F32, engine=_lib.ENGINE_WGMMA, out_nchw=1, pow_channel=0).cpu()
     ref = conv_ref(x, w, b, pow_channel=0).permute(0, 3, 1, 2)
     assert torch.allclose(got, ref, rtol=2e-5, atol=2e-4)
 
@@ -80,7 +80,7 @@ def test_tcgen05_stem_u8(B, H, W):
     x = torch.from_numpy(rs.randint(0, 256, (B, H, W, 3)).astype(np.uint8)).cuda()
     w = rs.normal(0, 0.2, (64, 3, 3, 3)).astype(np.float32)
     b = rs.normal(0, 0.5, 64).astype(np.float32)
-    got = conv2d(x, w, b, stride=2, relu=True, out_dtype=BF16, engine=_lib.ENGINE_TCGEN05, input_norm=1).float().cpu()
+    got = conv2d(x, w, b, stride=2, relu=True, out_dtype=BF16, engine=_lib.ENGINE_WGMMA, input_norm=1).float().cpu()
     # the engine rounds w * 2/255 to bf16; use exactly those weights in the reference
     w_eff = (torch.from_numpy(w * (2.0 / 255.0)).bfloat16().float() * (255.0 / 2.0)).numpy()
     ref = conv_ref(x, w_eff, b, stride=2, relu=True, input_norm=1)
@@ -96,7 +96,7 @@ def test_tcgen05_conv1d_streamed_weights(cin, cout, B, out_bf16):
     x = torch.from_numpy(rs.normal(0, 1, (B, 1, 128, cin)).astype(np.float32)).cuda().bfloat16()
     w = torch.from_numpy(rs.normal(0, 1 / np.sqrt(cin * 3), (cout, cin, 3)).astype(np.float32)).bfloat16().float().numpy()
     b = rs.normal(0, 0.5, cout).astype(np.float32)
-    got = conv2d(x, w, b, relu=True, out_dtype=BF16 if out_bf16 else F32, engine=_lib.ENGINE_TCGEN05).float().cpu()
+    got = conv2d(x, w, b, relu=True, out_dtype=BF16 if out_bf16 else F32, engine=_lib.ENGINE_WGMMA).float().cpu()
     ref = conv_ref(x, w, b, relu=True)
     tol = 3e-4 + (2.0 ** -8) * ref.abs() if out_bf16 else 3e-4 + 1e-5 * ref.abs()
     bad = (got - ref).abs() > tol
@@ -111,7 +111,7 @@ def test_bf16_rounding_error_of_one_layer_is_bounded(k, cin, cout, hw):
     rs = np.random.RandomState(k * 1000 + cin)
     x = rs.normal(0, 1, (2, hw, hw, cin)).astype(np.float32)
     w = rs.normal(0, 1 / np.sqrt(cin * k * k), (cout, cin, k, k)).astype(np.float32)
-    got = conv2d(torch.from_numpy(x).cuda().bfloat16(), w, None, out_dtype=BF16, engine=_lib.ENGINE_TCGEN05).float().cpu()
+    got = conv2d(torch.from_numpy(x).cuda().bfloat16(), w, None, out_dtype=BF16, engine=_lib.ENGINE_WGMMA).float().cpu()
     ref = conv_ref(torch.from_numpy(x), w)
     rel = float((got - ref).norm() / ref.norm())
     print(f"k{k} {cin}->{cout}: relative L2 error of the bf16 layer {rel:.2e}")
