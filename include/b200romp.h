@@ -10,8 +10,8 @@
  * input/output buffers; the library owns only packed constants and the conv-graph workspace.
  *
  * Device selection: entry points that take a handle (net, smpl, bev, tracks) make the handle's device current themselves;
- * the handle-less ones (parse, project, preprocess_bgr, pack_rows, bev_bv_input / parse3d / post / crop_post / long_merge,
- * gather_rows) launch on
+ * the handle-less ones (parse, project / project_frames, preprocess_bgr / preprocess_bgr_batch, pack_rows, bev_bv_input /
+ * parse3d / post / post_frames / crop_post / long_merge, gather_rows) launch on
  * the CURRENT device - the caller must have made the device that owns the stream and the buffers current.
  *
  * Return convention: 0 = OK, negative = error (b200romp_last_error() gives the text).  "Nobody
@@ -183,6 +183,13 @@ int b200romp_project(const float* joints /*[n,71,3]*/, const float* verts /*[n,6
                      int n, const int* d_count, const float* offsets6, float* pj2d_org /*[n,71,2]*/,
                      float* verts_camed_org /*[n,6890,3] or NULL*/, float* cam_trans_weak /*[n,3] or NULL*/,
                      float* cam_trans_lsq /*[n,3] or NULL*/, b200romp_stream stream);
+/* The same outputs for a batch of frames of different sizes: person i's pj2d_org / verts_camed_org use the pad info of its
+ * frame, row batch_ids[i] of pad_table = DEVICE fp32 [B,6] [top,bottom,left,right,h,w] (as b200romp_preprocess_bgr_batch
+ * writes it) - convert_proejection_from_input_to_orgimg (post_parser.py:81-88) with each image's own offsets, as the
+ * reference's one-image call (main.py:160-176) applies them.  cam_trans does not depend on the pad info. */
+int b200romp_project_frames(const float* joints, const float* verts, const float* cam, int n, const int* d_count,
+                            const long long* batch_ids /*[n]*/, const float* pad_table, float* pj2d_org, float* verts_camed_org,
+                            float* cam_trans_weak, float* cam_trans_lsq, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
  * BEV variant (simple_romp/bev): the stages of BEVv1.forward (bev/model.py:232-250) and of
@@ -231,6 +238,14 @@ int b200romp_bev_post(const float* betas, const float* verts_smil, const float* 
                       const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
                       const int* d_count, const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side,
                       float* pj2d_org, int* keep, int* sel, int* d_count_out, b200romp_stream stream);
+/* b200romp_bev_post for a batch of frames of different sizes: the host offsets6 / img_max_side are replaced by the DEVICE
+ * fp32 [batch,6] pad_table ([top,bottom,left,right,h,w] per frame).  Each frame projects with its own size, left and top
+ * (bev/post_parser.py:129-152) and suppresses with its own threshold nms_thresh * max(h,w) / 640 (:148-149,186-187) - what
+ * BEV.process_normal_image (bev/main.py:158-181) does for one image. */
+int b200romp_bev_post_frames(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                             const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
+                             const int* d_count, const float* pad_table, float nms_thresh, float rel_scale_thresh, float* pj2d_org,
+                             int* keep, int* sel, int* d_count_out, b200romp_stream stream);
 /* Long-image (crowd) mode, per-crop stage (bev/main.py:196-249, bev/split2process.py:41-58) for one chunk of crop frames
  * (batch frames = crops crop0 .. crop0+batch-1 of the image, rows grouped by frame like bev_parse3d leaves them).  After
  * SMPL-A / SMIL: merge babies, then per crop: drop the persons in the overlap with the neighbouring crops (cam x against
@@ -269,6 +284,13 @@ int b200romp_gather_rows(const void* src, int row_bytes, const int* sel, const i
  * pad_info6 (HOST, may be NULL) receives [top, bottom, left, right, h, w] like padding_image. */
 int b200romp_preprocess_bgr(const unsigned char* img_bgr_device, int h, int w, int row_stride_bytes, int out_size,
                             unsigned char* out_rgb_device, float* pad_info6_host, b200romp_stream stream);
+/* The same for n raw BGR images of different sizes (a folder of photos, the crops of a wide image: the reference
+ * preprocesses each with its own img_preprocess call, main.py:161, bev/main.py:160,197-199): image i is the DEVICE pointer
+ * imgs_bgr[i] with h[i] x w[i] pixels and a row stride of row_stride_bytes[i] bytes - all four are HOST arrays - and becomes
+ * out_rgb_device[i] of [n, out_size, out_size, 3].  pad_table (DEVICE fp32 [n,6], may be NULL) receives each image's
+ * [top, bottom, left, right, h, w].  One launch per 64 images; b200romp_preprocess_bgr is its n = 1 case. */
+int b200romp_preprocess_bgr_batch(const unsigned char* const* imgs_bgr, const int* h, const int* w, const int* row_stride_bytes,
+                                  int n, int out_size, unsigned char* out_rgb_device, float* pad_table, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Row f4: the temporal stage of ROMP.forward with --temporal_optimize (main.py:117-157): One-Euro smoothing of

@@ -145,6 +145,7 @@ def load():
     _sig(lib.b200romp_smpl_workspace_floats, i32)
     _sig(lib.b200romp_smpl_forward, i32, vp, vp, i32, vp, i32, vp, i32, vp, vp, vp, vp)
     _sig(lib.b200romp_project, i32, vp, vp, vp, i32, vp, fp, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_project_frames, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_create, vp, i32, C.POINTER(BevWeights))
     _sig(lib.b200romp_bev_destroy, None, vp)
     _sig(lib.b200romp_bev_bv_input, i32, vp, vp, i32, i32, i32, vp, i32, vp)
@@ -153,6 +154,7 @@ def load():
     _sig(lib.b200romp_bev_parse3d, i32, vp, i32, f32, i32, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_regress, i32, vp, vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_post, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_bev_post_frames, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, f32, f32, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_crop_post, i32, *([vp] * 11), i32, i32, vp, vp, i32, f32, vp, vp, vp, vp, i32, *([vp] * 9), vp)
     _sig(lib.b200romp_bev_long_merge_workspace_bytes, i64, i32)
     _sig(lib.b200romp_bev_long_merge, i32, vp, vp, vp, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp, vp, vp)
@@ -162,6 +164,7 @@ def load():
     _sig(lib.b200romp_tracks_reset, i32, vp, i32, vp)
     _sig(lib.b200romp_one_euro_smooth, i32, vp, vp, i32, vp, vp, vp, i32, i32, vp, f32, f32, vp)
     _sig(lib.b200romp_preprocess_bgr, i32, vp, i32, i32, i32, i32, vp, fp, vp)
+    _sig(lib.b200romp_preprocess_bgr_batch, i32, C.POINTER(vp), ip, ip, ip, i32, i32, vp, vp, vp)
     _sig(lib.b200romp_pack_rows, i32, C.POINTER(vp), ip, i32, vp, i32, i32, i32, i32, vp, i32, vp)
     if lib.b200romp_version() != 200:
         raise RuntimeError("libb200romp.so version mismatch - rebuild")
@@ -184,10 +187,11 @@ EXPORTS = [
     "b200romp_net_describe", "b200romp_net_num_launches", "b200romp_net_workspace_bytes", "b200romp_net_profile",
     "b200romp_conv2d",
     "b200romp_parse", "b200romp_parse_workspace_bytes", "b200romp_smpl_create", "b200romp_smpl_destroy",
-    "b200romp_smpl_workspace_floats", "b200romp_smpl_forward", "b200romp_project",
+    "b200romp_smpl_workspace_floats", "b200romp_smpl_forward", "b200romp_project", "b200romp_project_frames",
     "b200romp_bev_create", "b200romp_bev_destroy", "b200romp_bev_bv_input", "b200romp_bev_center3d",
     "b200romp_bev_parse_workspace_bytes", "b200romp_bev_parse3d", "b200romp_bev_regress", "b200romp_bev_post",
-    "b200romp_bev_crop_post", "b200romp_bev_long_merge_workspace_bytes", "b200romp_bev_long_merge",
-    "b200romp_gather_rows", "b200romp_pack_rows", "b200romp_preprocess_bgr", "b200romp_tracks_create", "b200romp_tracks_destroy",
+    "b200romp_bev_post_frames", "b200romp_bev_crop_post", "b200romp_bev_long_merge_workspace_bytes", "b200romp_bev_long_merge",
+    "b200romp_gather_rows", "b200romp_pack_rows", "b200romp_preprocess_bgr", "b200romp_preprocess_bgr_batch",
+    "b200romp_tracks_create", "b200romp_tracks_destroy",
     "b200romp_tracks_reset", "b200romp_one_euro_smooth",
 ]

@@ -4,7 +4,8 @@
 True and therefore overrides the thresholds with ``long_conf_dict``), ``BEV(settings)(image_bgr) -> dict | None``
 mirrors bev/main.py:91-258: normal images run as one 512x512 frame, and in crowd mode images at least twice as wide as
 high run through ``process_long_image`` (the reference's overlapping crops, batched through the model, with the per-crop
-and merged filters on the device).  ``forward_batch`` is the batched entry point for normal frames.
+and merged filters on the device).  ``forward_batch`` is the batched entry point for normal frames, ``forward_images`` the
+batched ``forward`` on raw images of different sizes (each frame with its own geometry).
 Per-frame semantics of the two post filters (bev/post_parser.py:167-222) are preserved by applying them per
 ``pred_batch_ids`` group on the device.  Python only allocates buffers and sequences library calls.
 """
@@ -21,7 +22,8 @@ import torch
 
 from . import _lib, graph
 from ._lib import BF16, F32, U8
-from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
+from .main import (MAX_PERSON, SMPLParser, _ptr, image_tensor, img_preprocess, preprocess_bgr_batch, split_by_frame, stage_host_images,
+                   staging_layout)
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
 long_conf_dict = {1: [0.12, 20, 1.5, 0.46], 2: [0.08, 20, 1.6, 0.8]}
@@ -186,6 +188,8 @@ class BEV(torch.nn.Module):
         if self.calc_smpl:
             self.out.update(verts=torch.zeros_like(self.buf["verts"]), joints=torch.zeros_like(self.buf["joints"]))
         self.count_host = torch.zeros(2, dtype=torch.int32).pin_memory()
+        self.pad_table = z(B, 6)                       # per-frame pad info of forward_images / forward_batch([B,6] offsets)
+        self._raw_host = self._raw_dev = None           # raw image staging of forward_images (grown on demand)
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -220,20 +224,27 @@ class BEV(torch.nn.Module):
 
     @torch.no_grad()
     def run_post(self, B, offsets, img_max_side=512.0):
-        """SMPLA_parser + projection + the two per-frame filters (bev/main.py:172-180), then row compaction."""
+        """SMPLA_parser + projection + the two per-frame filters (bev/main.py:172-180), then row compaction.  ``offsets``:
+        one pad info for every frame (suppression with ``img_max_side``), or a device [B,6] table with one row per frame
+        (each frame projects and suppresses with its own size)."""
         lib, b, o, sp = self.lib, self.buf, self.out, C.c_void_p(self.stream.cuda_stream)
         cap = B * MAX_PERSON
-        off = (C.c_float * 6)(*[float(v) for v in offsets])
         if not self.calc_smpl:
             return
         st = self.stream.cuda_stream
         self.smpla.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts"], b["joints"], st)
         self.smil.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts_smil"], b["joints_smil"], st)
-        _lib.check(lib.b200romp_bev_post(_ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]),
-                                         _ptr(b["joints"]), _ptr(b["cam"]), _ptr(b["cam_trans"]), _ptr(b["batch_ids"]), B, cap,
-                                         _ptr(b["count"]), off, float(self.settings.nms_thresh),
-                                         float(self.settings.relative_scale_thresh), float(img_max_side), _ptr(b["pj2d_org"]),
-                                         _ptr(b["keep"]), _ptr(b["sel"]), _ptr(b["count2"]), sp), "bev_post")
+        args = (_ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]), _ptr(b["joints"]), _ptr(b["cam"]),
+                _ptr(b["cam_trans"]), _ptr(b["batch_ids"]), B, cap, _ptr(b["count"]))
+        if isinstance(offsets, torch.Tensor) and offsets.dim() == 2:
+            _lib.check(lib.b200romp_bev_post_frames(*args, _ptr(offsets), float(self.settings.nms_thresh),
+                                                    float(self.settings.relative_scale_thresh), _ptr(b["pj2d_org"]), _ptr(b["keep"]),
+                                                    _ptr(b["sel"]), _ptr(b["count2"]), sp), "bev_post_frames")
+        else:
+            off = (C.c_float * 6)(*[float(v) for v in offsets])
+            _lib.check(lib.b200romp_bev_post(*args, off, float(self.settings.nms_thresh), float(self.settings.relative_scale_thresh),
+                                             float(img_max_side), _ptr(b["pj2d_org"]), _ptr(b["keep"]), _ptr(b["sel"]),
+                                             _ptr(b["count2"]), sp), "bev_post")
         for k, dst in o.items():
             src = b["conf"] if k == "conf" else b[k]
             row = src[0].numel() * src.element_size()
@@ -264,12 +275,15 @@ class BEV(torch.nn.Module):
 
     @torch.no_grad()
     def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0):
+        """frames [B,512,512,3] padded+resized like img_preprocess.  ``offsets``: one pad info [top,bottom,left,right,h,w]
+        for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
+        suppressing with its own max(h, w) (``img_max_side`` is not used)."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         B = frames.shape[0]
         # device-resident inputs come from the caller's current stream: order self.stream after it (no host sync)
         cur = torch.cuda.current_stream(self.tdevice)
-        for t in (frames, center3d_override):
+        for t in (frames, center3d_override, offsets):
             if isinstance(t, torch.Tensor) and t.is_cuda:
                 if cur != self.stream:
                     self.stream.wait_stream(cur)
@@ -280,9 +294,86 @@ class BEV(torch.nn.Module):
         fd = self._staging[key]
         with torch.cuda.stream(self.stream):
             fd.copy_(frames, non_blocking=True)
+            if offsets is not None and np.ndim(offsets) == 2:
+                assert tuple(np.shape(offsets)) == (B, 6), "per-frame offsets must be [B,6]"
+                offsets = self.pad_table[:B].copy_(torch.as_tensor(np.asarray(offsets, np.float32) if not isinstance(offsets, torch.Tensor)
+                                                                   else offsets.float()))
             self.run_model(fd, center3d_override)
             self.run_post(B, offsets if offsets is not None else [0, 512, 0, 512, 512, 512], img_max_side)
         return self.collect(to_numpy)
+
+    @torch.no_grad()
+    def forward_images(self, images, to_numpy=True, center3d_override=None):
+        """Batched ``forward`` on raw images of any sizes (HxWx3 uint8 BGR: numpy arrays, host or device tensors): a list
+        of the same length, element i the result for images[i] (dict or None; nothing is printed for normal images).
+        Normal images run in chunks of at most ``max_batch`` through one preprocessing kernel per chunk (the GPU kernel,
+        not the host OpenCV resize of ``forward``) and b200romp_bev_post_frames, each frame with its own pad info and
+        suppression threshold; element i then equals ``forward_batch`` on image i's GPU-preprocessed frame with its pad
+        info and ``img_max_side = max(h, w)``.  In crowd mode images with w/h >= 2 go one by one through
+        ``process_long_image``.  center3d_override: optional device [n_normal,64,128,128] for the normal images in order."""
+        imgs = [image_tensor(x) for x in images]
+        res = [None] * len(imgs)
+        normal = []
+        for i, t in enumerate(imgs):
+            if self.settings.crowd and t.shape[1] / t.shape[0] >= 2:
+                if getattr(self.settings, "show_patch_results", False):
+                    raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
+                res[i] = self.process_long_image(t, to_numpy=to_numpy)
+            else:
+                normal.append(i)
+        if center3d_override is not None:
+            assert center3d_override.is_cuda and center3d_override.shape[0] == len(normal)
+            if torch.cuda.current_stream(self.tdevice) != self.stream:
+                self.stream.wait_stream(torch.cuda.current_stream(self.tdevice))
+            center3d_override.record_stream(self.stream)
+        for c0 in range(0, len(normal), self.max_batch):
+            idx = normal[c0:c0 + self.max_batch]
+            for i, r in zip(idx, self._forward_chunk([imgs[i] for i in idx], to_numpy,
+                                                     None if center3d_override is None else center3d_override[c0:c0 + len(idx)])):
+                res[i] = r
+        return res
+
+    def _forward_chunk(self, imgs, to_numpy, center3d_override):
+        """One chunk of normal images: staging + one H2D, batched preprocessing, model, per-frame post; one host sync."""
+        B = len(imgs)
+        offs, total = staging_layout(imgs)
+        if total and (self._raw_host is None or self._raw_host.numel() < total):
+            self.stream.synchronize()                       # the previous chunk's preprocessing no longer reads the old buffers
+            self._raw_host = torch.empty(max(total, 1 << 24), dtype=torch.uint8).pin_memory()
+            self._raw_dev = torch.empty(self._raw_host.numel(), dtype=torch.uint8, device=self.tdevice)
+        stage_host_images(imgs, offs, self._raw_host)        # the previous chunk ended in a host sync: the buffer is free
+        cur = torch.cuda.current_stream(self.tdevice)
+        for t in imgs:
+            if t.is_cuda:
+                if cur != self.stream:
+                    self.stream.wait_stream(cur)
+                t.record_stream(self.stream)
+        key = (torch.uint8, B)
+        if key not in self._staging:
+            self._staging[key] = torch.empty((B, 512, 512, 3), dtype=torch.uint8, device=self.tdevice)
+        fd = self._staging[key]
+        with torch.cuda.stream(self.stream):
+            if total:
+                self._raw_dev[:total].copy_(self._raw_host[:total], non_blocking=True)
+            preprocess_bgr_batch(self.lib, imgs, offs, self._raw_dev, fd, self.pad_table, self.stream.cuda_stream)
+            self.run_model(fd, center3d_override)
+            self.run_post(B, self.pad_table[:B])
+        out = self.collect(to_numpy)
+        if out is None:
+            return [None] * B
+        n_det = int(self.count_host[0])
+        detected = set(self.buf["batch_ids"][:n_det].cpu().tolist())       # frames with a detection (before the filters)
+        ids = out["pred_batch_ids"]
+        ids = ids.cpu().numpy() if isinstance(ids, torch.Tensor) else ids
+        res = []
+        for i, (a, b) in enumerate(split_by_frame(ids, B)):
+            if i not in detected:                          # forward_batch on this frame alone returns None
+                res.append(None)
+                continue
+            r = {k: (np.array(v[a:b]) if to_numpy else v[a:b].clone()) for k, v in out.items()}
+            r["pred_batch_ids"] = np.zeros(b - a, np.int64) if to_numpy else torch.zeros(b - a, dtype=torch.int64, device=self.tdevice)
+            res.append(r)
+        return res
 
     def _long_buffers(self, rows):
         """Image-level accumulation rows of the long-image mode (grown on demand, kept for the next image)."""
@@ -352,12 +443,10 @@ class BEV(torch.nn.Module):
         return padded
 
     def crop_frames(self, padded, boxes, frames):
-        """frames[i] = img_preprocess(padded[t:b, l:r]) for box i: one b200romp_preprocess_bgr per crop on its window of the
-        padded image (pointer offset, the crop's own size, the padded row stride)."""
-        W, sp = int(padded.shape[1]), C.c_void_p(self.stream.cuda_stream)
-        for i, (l, r, t, b) in enumerate(np.asarray(boxes).tolist()):
-            _lib.check(self.lib.b200romp_preprocess_bgr(C.c_void_p(padded.data_ptr() + (t * W + l) * 3), b - t, r - l, 3 * W, 512,
-                                                        C.c_void_p(frames[i].data_ptr()), None, sp), "preprocess_bgr")
+        """frames[i] = img_preprocess(padded[t:b, l:r]) for box i: one b200romp_preprocess_bgr_batch call for all the boxes,
+        each crop a window of the padded image (its own size, the padded row stride)."""
+        crops = [padded[t:b, l:r] for l, r, t, b in np.asarray(boxes).tolist()]
+        preprocess_bgr_batch(self.lib, crops, [None] * len(crops), None, frames, None, self.stream.cuda_stream)
 
     def crop_post(self, nb, crop0, tab_dev):
         """SMPL-A / SMIL on the chunk's persons, then the per-crop stage (b200romp_bev_crop_post): survivors appended to

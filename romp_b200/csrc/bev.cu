@@ -373,11 +373,19 @@ __global__ void __launch_bounds__(256) bev_merge_smil_kernel(const float* __rest
     for (int i = threadIdx.x; i < 213; i += 256) joints[(size_t)n * 213 + i] = joints_smil[(size_t)n * 213 + i];
 }
 
+// pad_tab (device [B,6] fp32 [top,bottom,left,right,h,w] per frame, may be NULL): person n projects with the row of its
+// frame batch_ids[n] instead of the shared size / left / top
 __global__ void __launch_bounds__(128) bev_project_kernel(const float* __restrict__ joints, const float* __restrict__ cam_trans,
                                                           const int* __restrict__ d_count, float size, float left, float top,
+                                                          const float* __restrict__ pad_tab, const long long* __restrict__ batch_ids,
                                                           float* __restrict__ pj2d_org) {
   const int n = blockIdx.x, j = threadIdx.x;
   if (n >= *d_count || j >= 71) return;
+  if (pad_tab) {
+    const float* f = pad_tab + batch_ids[n] * 6;
+    top = f[0]; left = f[2];
+    size = f[4] > f[5] ? f[4] : f[5];
+  }
   const float* q = joints + ((size_t)n * 71 + j) * 3;
   const float px = q[0] + cam_trans[n * 3], py = q[1] + cam_trans[n * 3 + 1], pz = q[2] + cam_trans[n * 3 + 2];
   const float iz = pz + 1e-6f;
@@ -462,11 +470,15 @@ __device__ void postfilter_frame(const float* __restrict__ pj2d_org, const float
 __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
                                                              const float* __restrict__ cam_trans, const long long* __restrict__ batch_ids,
                                                              const int* __restrict__ d_count, float nms_thr_px, float rel_scale_thresh,
-                                                             int* __restrict__ keep) {
+                                                             const float* __restrict__ pad_tab, float nms_thresh, int* __restrict__ keep) {
   __shared__ int s_start, s_n;
   __shared__ int s_drop[kMaxP], s_removed[kMaxP], s_kept[kMaxP], s_nk;
   __shared__ float s_mean[kMaxP];
   const int b = blockIdx.x, tid = threadIdx.x;
+  if (pad_tab) {                       // this frame's own threshold nms_thresh * max(h, w) / 640 (bev/post_parser.py:186-187)
+    const float h = pad_tab[b * 6 + 4], w = pad_tab[b * 6 + 5];
+    nms_thr_px = __fdiv_rn(__fmul_rn(nms_thresh, h > w ? h : w), 640.f);
+  }
   if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n);
   if (tid < kMaxP) s_drop[tid] = 0;
   __syncthreads();
@@ -853,23 +865,44 @@ int b200romp_bev_regress(b200romp_bev* h, const float* maps_fv, const void* bv_o
   return B200ROMP_OK;
 }
 
+static int bev_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints, const float* cam,
+                    const float* cam_trans, const long long* batch_ids, int batch, int capacity, const int* d_count, const float* offsets6,
+                    const float* pad_table, float nms_thresh, float rel_scale_thresh, float img_max_side, float* pj2d_org, int* keep,
+                    int* sel, int* d_count_out, cudaStream_t stream) {
+  if (verts_smil && joints_smil)
+    bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
+  float top = 0.f, left = 0.f, size = 0.f;
+  if (offsets6) {
+    const float hh = offsets6[4], ww = offsets6[5];
+    top = offsets6[0]; left = offsets6[2]; size = hh > ww ? hh : ww;
+  }
+  bev_project_kernel<<<capacity, 128, 0, stream>>>(joints, cam_trans, d_count, size, left, top, pad_table, batch_ids, pj2d_org);
+  B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
+  bev_postfilter_kernel<<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
+                                                   rel_scale_thresh, pad_table, nms_thresh, keep);
+  bev_compact_kernel<<<1, 32, 0, stream>>>(keep, d_count, sel, d_count_out);
+  B2R_CUDA_OK(cudaGetLastError());
+  return B200ROMP_OK;
+}
+
 int b200romp_bev_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                       const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
                       const int* d_count, const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side,
                       float* pj2d_org, int* keep, int* sel, int* d_count_out, b200romp_stream stream_) {
   B2R_REQUIRE(betas && verts && joints && cam && cam_trans && batch_ids && d_count && offsets6 && pj2d_org && keep && sel &&
                   d_count_out && batch > 0 && capacity > 0, "bev_post: bad arguments");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (verts_smil && joints_smil)
-    bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
-  const float top = offsets6[0], left = offsets6[2], hh = offsets6[4], ww = offsets6[5];
-  bev_project_kernel<<<capacity, 128, 0, stream>>>(joints, cam_trans, d_count, hh > ww ? hh : ww, left, top, pj2d_org);
-  B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
-  bev_postfilter_kernel<<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
-                                                   rel_scale_thresh, keep);
-  bev_compact_kernel<<<1, 32, 0, stream>>>(keep, d_count, sel, d_count_out);
-  B2R_CUDA_OK(cudaGetLastError());
-  return B200ROMP_OK;
+  return bev_post(betas, verts_smil, joints_smil, verts, joints, cam, cam_trans, batch_ids, batch, capacity, d_count, offsets6, nullptr,
+                  nms_thresh, rel_scale_thresh, img_max_side, pj2d_org, keep, sel, d_count_out, (cudaStream_t)stream_);
+}
+
+int b200romp_bev_post_frames(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                             const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
+                             const int* d_count, const float* pad_table, float nms_thresh, float rel_scale_thresh, float* pj2d_org,
+                             int* keep, int* sel, int* d_count_out, b200romp_stream stream_) {
+  B2R_REQUIRE(betas && verts && joints && cam && cam_trans && batch_ids && d_count && pad_table && pj2d_org && keep && sel &&
+                  d_count_out && batch > 0 && capacity > 0, "bev_post_frames: bad arguments");
+  return bev_post(betas, verts_smil, joints_smil, verts, joints, cam, cam_trans, batch_ids, batch, capacity, d_count, nullptr, pad_table,
+                  nms_thresh, rel_scale_thresh, 0.f, pj2d_org, keep, sel, d_count_out, (cudaStream_t)stream_);
 }
 
 int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,

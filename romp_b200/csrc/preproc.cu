@@ -1,6 +1,8 @@
 // Row a1 / f2: img_preprocess + padding_image (simple_romp/romp/utils.py:16-30) on the GPU:
 //   cv2.cvtColor(BGR2RGB) -> centre zero-pad to a square -> cv2.resize(..., (S,S), INTER_CUBIC) -> uint8 [S,S,3]
-// in ONE kernel reading the raw BGR image and writing the network's input frame.
+// in ONE kernel reading the raw BGR image and writing the network's input frame.  One launch covers up to 64 images of
+// different sizes (grid z = image), each with its own padded square and scale, and writes each image's pad info to a
+// device table the per-frame post stages read.
 //
 // Bit-exactness target: OpenCV's own 8-bit bicubic resize (modules/imgproc/src/resize.cpp, the algorithm restated from
 // its published source; pip wheels additionally carry a closed-source IPP fast path whose results differ from OpenCV's
@@ -35,14 +37,34 @@ __device__ __forceinline__ void cubic_taps(int d, double scale, int* s0, int (&w
   *s0 = s;
 }
 
-// thread = one output pixel (3 channels)
-__global__ void __launch_bounds__(256) preprocess_bgr_kernel(const unsigned char* __restrict__ img, int h, int w, int row_stride, int side,
-                                                             int top, int left, double scale, int S, unsigned char* __restrict__ out) {
+// One image of a batch: device pointer, size, row stride, padded square and its resize scale (host-computed, so the
+// arithmetic is that of the single-image case).  A batch travels to the kernel as a launch parameter (no descriptor table
+// in device memory, no H2D copy).
+struct PreprocImage {
+  const unsigned char* img;
+  int h, w, row_stride, side, top, left;
+  double scale;
+};
+constexpr int kPreprocBatch = 64;     // images per launch: 64 x 40 B of descriptors stay well inside the 4 KB parameter space
+struct PreprocBatch { PreprocImage im[kPreprocBatch]; };
+
+// thread = one output pixel (3 channels) of image blockIdx.z; pad_tab (device [n,6] fp32, may be NULL) receives each
+// image's [top, bottom, left, right, h, w] (utils.py:24)
+__global__ void __launch_bounds__(256) preprocess_bgr_kernel(const __grid_constant__ PreprocBatch batch, int S,
+                                                             unsigned char* __restrict__ out, float* __restrict__ pad_tab) {
+  const PreprocImage& im = batch.im[blockIdx.z];
   const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y;
+  if (pad_tab && dx == 0 && dy == 0) {
+    float* p = pad_tab + (size_t)blockIdx.z * 6;
+    p[0] = (float)im.top; p[1] = (float)(im.top + im.h); p[2] = (float)im.left; p[3] = (float)(im.left + im.w);
+    p[4] = (float)im.h; p[5] = (float)im.w;
+  }
   if (dx >= S) return;
+  const unsigned char* __restrict__ img = im.img;
+  const int h = im.h, w = im.w, row_stride = im.row_stride, side = im.side, top = im.top, left = im.left;
   int sx, sy, ax[4], ay[4];
-  cubic_taps(dx, scale, &sx, ax);
-  cubic_taps(dy, scale, &sy, ay);
+  cubic_taps(dx, im.scale, &sx, ax);
+  cubic_taps(dy, im.scale, &sy, ay);
   int rows[4][3];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -62,7 +84,7 @@ __global__ void __launch_bounds__(256) preprocess_bgr_kernel(const unsigned char
   }
   const float sc = 1.f / (2048.f * 2048.f);
   const float b0 = __fmul_rn((float)ay[0], sc), b1 = __fmul_rn((float)ay[1], sc), b2 = __fmul_rn((float)ay[2], sc), b3 = __fmul_rn((float)ay[3], sc);
-  unsigned char* o = out + ((size_t)dy * S + dx) * 3;
+  unsigned char* o = out + (((size_t)blockIdx.z * S + dy) * S + dx) * 3;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     float t = __fmul_rn((float)rows[3][c], b3);
@@ -73,22 +95,44 @@ __global__ void __launch_bounds__(256) preprocess_bgr_kernel(const unsigned char
   }
 }
 
+static PreprocImage preproc_image(const unsigned char* img, int h, int w, int row_stride, int out_size) {
+  PreprocImage im;
+  im.img = img; im.h = h; im.w = w; im.row_stride = row_stride;
+  im.side = h > w ? h : w;
+  im.top = (im.side - h) / 2; im.left = (im.side - w) / 2;
+  im.scale = (double)im.side / (double)out_size;
+  return im;
+}
+
 }  // namespace b200romp
 
 using namespace b200romp;
 
+extern "C" int b200romp_preprocess_bgr_batch(const unsigned char* const* imgs_bgr, const int* h, const int* w, const int* row_stride_bytes,
+                                             int n, int out_size, unsigned char* out_rgb, float* pad_table, b200romp_stream stream) {
+  B2R_REQUIRE(imgs_bgr && h && w && row_stride_bytes && n > 0 && out_size > 0 && out_rgb, "preprocess_bgr_batch: bad arguments");
+  for (int i = 0; i < n; ++i)
+    B2R_REQUIRE(imgs_bgr[i] && h[i] > 0 && w[i] > 0 && row_stride_bytes[i] >= 3 * w[i], "preprocess_bgr_batch: bad image");
+  const size_t frame = (size_t)out_size * out_size * 3;
+  for (int i0 = 0; i0 < n; i0 += kPreprocBatch) {
+    const int nb = n - i0 < kPreprocBatch ? n - i0 : kPreprocBatch;
+    PreprocBatch batch;
+    for (int i = 0; i < nb; ++i) batch.im[i] = preproc_image(imgs_bgr[i0 + i], h[i0 + i], w[i0 + i], row_stride_bytes[i0 + i], out_size);
+    dim3 grid((out_size + 255) / 256, out_size, nb);
+    preprocess_bgr_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(batch, out_size, out_rgb + i0 * frame,
+                                                                 pad_table ? pad_table + (size_t)i0 * 6 : nullptr);
+    B2R_CUDA_OK(cudaGetLastError());
+  }
+  return B200ROMP_OK;
+}
+
 extern "C" int b200romp_preprocess_bgr(const unsigned char* img_bgr, int h, int w, int row_stride_bytes, int out_size,
                                        unsigned char* out_rgb, float* pad_info6, b200romp_stream stream) {
   B2R_REQUIRE(img_bgr && out_rgb && h > 0 && w > 0 && row_stride_bytes >= 3 * w && out_size > 0, "preprocess_bgr: bad arguments");
-  const int side = h > w ? h : w;
-  const int top = (side - h) / 2, left = (side - w) / 2;
   if (pad_info6) {                     // utils.py:24: [top, bottom, left, right, h, w]
-    pad_info6[0] = (float)top; pad_info6[1] = (float)(top + h); pad_info6[2] = (float)left; pad_info6[3] = (float)(left + w);
+    const PreprocImage im = preproc_image(img_bgr, h, w, row_stride_bytes, out_size);
+    pad_info6[0] = (float)im.top; pad_info6[1] = (float)(im.top + h); pad_info6[2] = (float)im.left; pad_info6[3] = (float)(im.left + w);
     pad_info6[4] = (float)h; pad_info6[5] = (float)w;
   }
-  dim3 grid((out_size + 255) / 256, out_size);
-  preprocess_bgr_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(img_bgr, h, w, row_stride_bytes, side, top, left, (double)side / (double)out_size,
-                                                               out_size, out_rgb);
-  B2R_CUDA_OK(cudaGetLastError());
-  return B200ROMP_OK;
+  return b200romp_preprocess_bgr_batch(&img_bgr, &h, &w, &row_stride_bytes, 1, out_size, out_rgb, nullptr, stream);
 }

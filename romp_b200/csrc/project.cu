@@ -9,13 +9,21 @@
 
 namespace b200romp {
 
+// pad_tab (device [B,6] fp32 [top,bottom,left,right,h,w] per frame, may be NULL): person n uses the row of its frame
+// batch_ids[n] instead of the shared size / left / top
 __global__ void __launch_bounds__(256) project_points_kernel(const float* __restrict__ pts, const float* __restrict__ cam,
                                                              int n_host, const int* __restrict__ d_count, int npts,
                                                              int out_dim, float size, float left, float top,
+                                                             const float* __restrict__ pad_tab, const long long* __restrict__ batch_ids,
                                                              float* __restrict__ out) {
   const int n = blockIdx.x;
   const int N = d_count ? min(n_host, *d_count) : n_host;
   if (n >= N) return;
+  if (pad_tab) {
+    const float* f = pad_tab + batch_ids[n] * 6;
+    top = f[0]; left = f[2];
+    size = f[4] > f[5] ? f[4] : f[5];                         // post_parser.py:83
+  }
   const float s = cam[n * 3 + 0], tx = cam[n * 3 + 1], ty = cam[n * 3 + 2];
   for (int i = blockIdx.y * 256 + threadIdx.x; i < npts; i += gridDim.y * 256) {
     const float* q = pts + ((size_t)n * npts + i) * 3;
@@ -81,29 +89,49 @@ __global__ void __launch_bounds__(128) cam_trans_kernel(const float* __restrict_
   lsq[n * 3 + 0] = (float)x[0]; lsq[n * 3 + 1] = (float)x[1]; lsq[n * 3 + 2] = (float)x[2];
 }
 
+static int project(const float* joints, const float* verts, const float* cam, int n, const int* d_count, const float* offsets6,
+                   const long long* batch_ids, const float* pad_table, float* pj2d_org, float* verts_camed_org, float* cam_trans_weak,
+                   float* cam_trans_lsq, cudaStream_t stream) {
+  float top = 0.f, left = 0.f, size = 0.f;
+  if (offsets6) {
+    const float h = offsets6[4], w = offsets6[5];
+    top = offsets6[0]; left = offsets6[2];
+    size = h > w ? h : w;                                    // post_parser.py:83
+  }
+  if (cam_trans_weak || cam_trans_lsq) {
+    cam_trans_kernel<<<(n + 127) / 128, 128, 0, stream>>>(joints, cam, n, d_count, 443.4f, 512.f, cam_trans_weak, cam_trans_lsq);
+    B2R_CUDA_OK(cudaGetLastError());
+  }
+  if (pj2d_org) {
+    project_points_kernel<<<dim3(n, 1), 256, 0, stream>>>(joints, cam, n, d_count, 71, 2, size, left, top, pad_table, batch_ids, pj2d_org);
+    B2R_CUDA_OK(cudaGetLastError());
+  }
+  if (verts_camed_org) {
+    project_points_kernel<<<dim3(n, 4), 256, 0, stream>>>(verts, cam, n, d_count, 6890, 3, size, left, top, pad_table, batch_ids,
+                                                          verts_camed_org);
+    B2R_CUDA_OK(cudaGetLastError());
+  }
+  return B200ROMP_OK;
+}
+
 }  // namespace b200romp
 
 using namespace b200romp;
 
 extern "C" int b200romp_project(const float* joints, const float* verts, const float* cam, int n, const int* d_count,
                                 const float* offsets6, float* pj2d_org, float* verts_camed_org, float* cam_trans_weak,
-                                float* cam_trans_lsq, b200romp_stream stream_) {
+                                float* cam_trans_lsq, b200romp_stream stream) {
   B2R_REQUIRE(joints && cam && offsets6 && n > 0, "project: bad arguments");
   B2R_REQUIRE(!verts_camed_org || verts, "project: verts_camed_org requested without verts");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const float top = offsets6[0], left = offsets6[2], h = offsets6[4], w = offsets6[5];
-  const float size = h > w ? h : w;                          // post_parser.py:83
-  if (cam_trans_weak || cam_trans_lsq) {
-    cam_trans_kernel<<<(n + 127) / 128, 128, 0, stream>>>(joints, cam, n, d_count, 443.4f, 512.f, cam_trans_weak, cam_trans_lsq);
-    B2R_CUDA_OK(cudaGetLastError());
-  }
-  if (pj2d_org) {
-    project_points_kernel<<<dim3(n, 1), 256, 0, stream>>>(joints, cam, n, d_count, 71, 2, size, left, top, pj2d_org);
-    B2R_CUDA_OK(cudaGetLastError());
-  }
-  if (verts_camed_org) {
-    project_points_kernel<<<dim3(n, 4), 256, 0, stream>>>(verts, cam, n, d_count, 6890, 3, size, left, top, verts_camed_org);
-    B2R_CUDA_OK(cudaGetLastError());
-  }
-  return B200ROMP_OK;
+  return project(joints, verts, cam, n, d_count, offsets6, nullptr, nullptr, pj2d_org, verts_camed_org, cam_trans_weak, cam_trans_lsq,
+                 (cudaStream_t)stream);
+}
+
+extern "C" int b200romp_project_frames(const float* joints, const float* verts, const float* cam, int n, const int* d_count,
+                                       const long long* batch_ids, const float* pad_table, float* pj2d_org, float* verts_camed_org,
+                                       float* cam_trans_weak, float* cam_trans_lsq, b200romp_stream stream) {
+  B2R_REQUIRE(joints && cam && batch_ids && pad_table && n > 0, "project_frames: bad arguments");
+  B2R_REQUIRE(!verts_camed_org || verts, "project_frames: verts_camed_org requested without verts");
+  return project(joints, verts, cam, n, d_count, nullptr, batch_ids, pad_table, pj2d_org, verts_camed_org, cam_trans_weak,
+                 cam_trans_lsq, (cudaStream_t)stream);
 }

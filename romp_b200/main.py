@@ -138,6 +138,53 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
+def image_tensor(image):
+    """HxWx3 uint8 BGR image (numpy, host or device tensor) -> a torch tensor the batched preprocessing can read: host
+    images as they are (they are copied into pinned staging), device images in place when their rows are packed BGR
+    pixels (any row stride >= 3w), else a contiguous copy."""
+    t = torch.from_numpy(np.ascontiguousarray(image)) if isinstance(image, np.ndarray) else image
+    assert isinstance(t, torch.Tensor) and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3, "image must be HxWx3 uint8 (BGR)"
+    assert t.shape[0] > 0 and t.shape[1] > 0, "empty image"
+    if t.is_cuda and not (t.stride(2) == 1 and t.stride(1) == 3 and t.stride(0) >= 3 * t.shape[1]):
+        t = t.contiguous()
+    return t
+
+
+def staging_layout(images):
+    """Byte offset of every host image inside one staging buffer (256-byte aligned; None for device images) and its size."""
+    offs, total = [], 0
+    for t in images:
+        offs.append(None if t.is_cuda else total)
+        if not t.is_cuda:
+            total += (t.numel() + 255) // 256 * 256
+    return offs, total
+
+
+def stage_host_images(images, offs, raw_host):
+    """Copy the host images into the pinned staging buffer (torch's copy_ splits each large copy over its CPU threads)."""
+    for t, o in zip(images, offs):
+        if o is not None:
+            raw_host[o:o + t.numel()].view(t.shape).copy_(t)
+
+
+def preprocess_bgr_batch(lib, images, offs, raw_dev, out, pad_table, stream):
+    """b200romp_preprocess_bgr_batch: images[i] (device tensor, or host tensor staged at raw_dev[offs[i]:]) -> out[i]
+    [512,512,3] uint8 RGB on the device, pad info into the device table pad_table [n,6] (may be None)."""
+    n = len(images)
+    ptrs = [t.data_ptr() if o is None else raw_dev.data_ptr() + o for t, o in zip(images, offs)]
+    strides = [t.stride(0) if o is None else 3 * int(t.shape[1]) for t, o in zip(images, offs)]
+    _lib.check(lib.b200romp_preprocess_bgr_batch((C.c_void_p * n)(*ptrs), (C.c_int * n)(*[int(t.shape[0]) for t in images]),
+                                                 (C.c_int * n)(*[int(t.shape[1]) for t in images]), (C.c_int * n)(*strides), n, 512,
+                                                 _ptr(out), None if pad_table is None else _ptr(pad_table), C.c_void_p(stream)),
+               "preprocess_bgr_batch")
+
+
+def split_by_frame(batch_ids, n_frames):
+    """Rows of a batch result grouped by frame (rows come in frame order): [(start, end)] per frame."""
+    b = np.searchsorted(np.asarray(batch_ids), np.arange(n_frames + 1))
+    return list(zip(b[:-1].tolist(), b[1:].tolist()))
+
+
 class SMPLParser:
     """Seam S3 (post_parser.SMPL_parser, post_parser.py:116-125) on libb200romp's fused SMPL kernels."""
 
@@ -265,7 +312,8 @@ class ROMP(torch.nn.Module):
             if self.calc_smpl:
                 d.update(verts=z(cap, 6890, 3), joints=z(cap, 71, 3))
             self.slots.append(dict(dev=d, host=None, count_host=torch.zeros(1, dtype=torch.int32).pin_memory(),
-                                   done=torch.cuda.Event(), frames={}, h2d=torch.cuda.Event()))
+                                   done=torch.cuda.Event(), frames={}, h2d=torch.cuda.Event(),
+                                   pad=z(B, 6), raw_host=None, raw_dev=None))   # per-frame pad info, raw image staging
         self._slot = 0
         self._raw_host = self._raw_dev = None
         self.copy_stream = torch.cuda.Stream(device=dev)
@@ -310,18 +358,25 @@ class ROMP(torch.nn.Module):
 
     @torch.no_grad()
     def run_smpl_project(self, cap, offsets, slot=None, count_on_device=True):
-        """Seams S3-S4 for up to ``cap`` persons (the device-side count limits it further unless count_on_device=False)."""
+        """Seams S3-S4 for up to ``cap`` persons (the device-side count limits it further unless count_on_device=False).
+        ``offsets``: one pad info [top,bottom,left,right,h,w] for every frame, or a device [B,6] table with one row per frame."""
         sh, lib, sp = self.shared, self.lib, C.c_void_p(self.stream.cuda_stream)
         b = (self.slots[self._slot] if slot is None else slot)["dev"]
         cnt = b["count"] if count_on_device else None
         cp = None if cnt is None else _ptr(cnt)
-        off = (C.c_float * 6)(*[float(v) for v in offsets])
+        per_frame = isinstance(offsets, torch.Tensor) and offsets.dim() == 2
+        off = (C.c_float * 6)(*[float(v) for v in ([0, 512, 0, 512, 512, 512] if per_frame else offsets)])
         if self.calc_smpl:
             self.smpl.forward(b["betas"], b["thetas"], cap, cnt, self.settings.root_align, sh["smpl_ws"],
                               b["verts"], b["joints"], self.stream.cuda_stream)
-            _lib.check(lib.b200romp_project(_ptr(b["joints"]), None, _ptr(b["cam"]), cap, cp, off,
-                                            _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp), "project")
-        else:   # without SMPL the reference keeps the weak-perspective translation of main.py:166
+            if per_frame:
+                _lib.check(lib.b200romp_project_frames(_ptr(b["joints"]), None, _ptr(b["cam"]), cap, cp, _ptr(b["batch_ids"]),
+                                                       _ptr(offsets), _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp),
+                           "project_frames")
+            else:
+                _lib.check(lib.b200romp_project(_ptr(b["joints"]), None, _ptr(b["cam"]), cap, cp, off,
+                                                _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp), "project")
+        else:   # without SMPL the reference keeps the weak-perspective translation of main.py:166 (no pad info involved)
             _lib.check(lib.b200romp_project(_ptr(b["cam"]), None, _ptr(b["cam"]), cap, cp, off, None, None,
                                             _ptr(b["cam_trans"]), None, sp), "project")
 
@@ -400,6 +455,8 @@ class ROMP(torch.nn.Module):
     def forward_batch(self, frames, offsets=None, to_numpy=True, center_override=None, own=True):
         """frames: [B,512,512,3] RGB uint8/float32 (torch tensor, pinned host or device, or numpy), already
         padded+resized like img_preprocess.  Returns the reference's dict plus ``pred_batch_ids`` or None.
+        ``offsets``: the pad info [top,bottom,left,right,h,w] of every frame, or one row per frame ([B,6], numpy or
+        tensor) when the frames come from images of different sizes.
         Device-resident ``frames`` / ``center_override`` may come straight from a producer on the caller's current
         stream.  ``own=True`` (default) returns arrays that own their memory; ``own=False`` returns views of the pinned
         read-back mirrors, valid until the second-next batch."""
@@ -408,10 +465,14 @@ class ROMP(torch.nn.Module):
         B = frames.shape[0]
         self._slot ^= 1
         slot = self.slots[self._slot]
-        self._after_producers(frames, center_override)
+        self._after_producers(frames, center_override, offsets)
         with torch.cuda.stream(self.stream):
             fd = self._staging(slot, frames.dtype, B)
             fd.copy_(frames, non_blocking=True)
+            if offsets is not None and np.ndim(offsets) == 2:
+                assert tuple(np.shape(offsets)) == (B, 6), "per-frame offsets must be [B,6]"
+                offsets = slot["pad"][:B].copy_(torch.as_tensor(np.asarray(offsets, np.float32) if not isinstance(offsets, torch.Tensor)
+                                                                else offsets.float()))
             self.run_maps(fd)
             self.run_post(B, offsets if offsets is not None else [0, 512, 0, 512, 512, 512], center_override)
             slot["done"].record(self.stream)
@@ -474,6 +535,92 @@ class ROMP(torch.nn.Module):
     def _read_back(self, slot, to_numpy=True):
         self.d2h_stream.wait_event(slot["done"])
         return self.collect(to_numpy, slot, self.d2h_stream)   # device views stay valid until the slot's next batch
+
+    @torch.no_grad()
+    def forward_images(self, images, to_numpy=True, center_override=None):
+        """Batched ``forward`` on raw images of any sizes: ``images`` is a sequence of HxWx3 uint8 BGR images (numpy arrays,
+        host or device tensors), run in chunks of at most ``max_batch``.  Returns a list of the same length whose element
+        i is what ``forward(images[i])`` returns (the reference's dict without ``pred_batch_ids``, or None; nothing is
+        printed).  center_override: optional device [n,1,64,64] replacing the images' center maps (tests, measurement)."""
+        return next(self.forward_image_batches([images], to_numpy, center_override))
+
+    @torch.no_grad()
+    def forward_image_batches(self, batches, to_numpy=True, center_override=None):
+        """Streaming form of ``forward_images`` over an iterable of image lists: yields one result list per input list, in
+        order.  Each chunk of at most ``max_batch`` images is staged into its slot's pinned buffer and sent with one H2D
+        on the copy stream (device images are read in place), preprocessed by one kernel into the slot's frames with
+        a per-frame pad table, and post-processed with each frame's own geometry; staging chunk i+1 and reading back
+        chunk i-1 overlap the kernels of chunk i (the two slots of ``forward_batches``).  center_override applies to
+        every list, entry k to the k-th image of the list."""
+        if self.temporal is not None:
+            raise NotImplementedError("--temporal_optimize smooths one image sequence: call forward() per frame")
+        self._after_producers(center_override)
+
+        def chunks():
+            for images in batches:
+                imgs = [image_tensor(x) for x in images]
+                res = [None] * len(imgs)
+                if not imgs:
+                    yield res, imgs, 0, True
+                for c0 in range(0, len(imgs), self.max_batch):
+                    yield res, imgs[c0:c0 + self.max_batch], c0, c0 + self.max_batch >= len(imgs)
+
+        pending = None
+        for res, imgs, c0, last in chunks():
+            co = None if center_override is None else center_override[c0:c0 + len(imgs)]
+            slot = self._submit_images(imgs, co) if imgs else None
+            if pending is not None:
+                done = self._finish_images(*pending, to_numpy)
+                if done is not None:
+                    yield done
+            pending = (slot, res, c0, len(imgs), last)
+        if pending is not None:
+            yield self._finish_images(*pending, to_numpy)
+
+    def _submit_images(self, imgs, center_override):
+        B = len(imgs)
+        self._slot ^= 1
+        slot = self.slots[self._slot]
+        fd = self._staging(slot, torch.uint8, B)
+        offs, total = staging_layout(imgs)
+        if total:
+            if slot["raw_host"] is None or slot["raw_host"].numel() < total:
+                slot["done"].synchronize()                 # the slot's previous kernels no longer read the old buffers
+                n = max(total, 1 << 24)
+                slot["raw_host"] = torch.empty(n, dtype=torch.uint8).pin_memory()
+                slot["raw_dev"] = torch.empty(n, dtype=torch.uint8, device=self.tdevice)
+            else:
+                slot["h2d"].synchronize()                  # the slot's previous H2D has left its pinned buffer
+            stage_host_images(imgs, offs, slot["raw_host"])
+            with torch.cuda.stream(self.copy_stream):
+                self.copy_stream.wait_event(slot["done"])  # the slot's previous preprocessing no longer reads raw_dev
+                slot["raw_dev"][:total].copy_(slot["raw_host"][:total], non_blocking=True)
+                slot["h2d"].record(self.copy_stream)
+        self._after_producers(*[t for t in imgs if t.is_cuda])
+        with torch.cuda.stream(self.stream):
+            if total:
+                self.stream.wait_event(slot["h2d"])
+            preprocess_bgr_batch(self.lib, imgs, offs, slot["raw_dev"], fd, slot["pad"], self.stream.cuda_stream)
+            self.run_maps(fd)
+            self.run_post(B, slot["pad"][:B], center_override, slot)
+            slot["done"].record(self.stream)
+        return slot
+
+    def _finish_images(self, slot, res, c0, B, last, to_numpy):
+        """Read back one chunk and scatter its persons to res[c0:c0+B]; returns res once its last chunk is in."""
+        out = None if slot is None else self._read_back(slot, to_numpy)
+        if out is not None:
+            ids = out["pred_batch_ids"]
+            ids = ids.cpu().numpy() if isinstance(ids, torch.Tensor) else ids
+            pnp = to_numpy and self.calc_smpl and getattr(self.settings, "cam_trans", "lsq") == "pnp"
+            for i, (a, b) in enumerate(split_by_frame(ids, B)):
+                if a == b:
+                    continue
+                r = {k: (np.array(v[a:b]) if to_numpy else v[a:b].clone()) for k, v in out.items() if k != "pred_batch_ids"}
+                if pnp:
+                    r["cam_trans"] = estimate_translation_pnp(r["joints"], r["cam"])
+                res[c0 + i] = r
+        return res if last else None
 
     @torch.no_grad()
     def preprocess(self, image, out=None):
