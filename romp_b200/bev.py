@@ -22,8 +22,8 @@ import torch
 
 from . import _lib, graph
 from ._lib import BF16, F32, U8
-from .main import (MAX_PERSON, SMPLParser, _ptr, image_tensor, img_preprocess, preprocess_bgr_batch, split_by_frame, stage_host_images,
-                   staging_layout)
+from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
+from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, split_by_frame
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
 long_conf_dict = {1: [0.12, 20, 1.5, 0.46], 2: [0.08, 20, 1.6, 0.8]}
@@ -133,7 +133,7 @@ class BEV(torch.nn.Module):
         self.tdevice = torch.device("cuda", self.device_index)
         torch.cuda.set_device(self.tdevice)
         self.precision = getattr(s, "precision", "bf16")
-        self._staging = {}
+        self._frames = {}                              # frame buffers by (dtype, B)
         self.max_batch = B = int(getattr(s, "max_batch", 32))
         if state_dict is None:
             state_dict = torch.load(s.model_path, map_location="cpu")          # bev/main.py:101 (strict=False)
@@ -189,7 +189,7 @@ class BEV(torch.nn.Module):
             self.out.update(verts=torch.zeros_like(self.buf["verts"]), joints=torch.zeros_like(self.buf["joints"]))
         self.count_host = torch.zeros(2, dtype=torch.int32).pin_memory()
         self.pad_table = z(B, 6)                       # per-frame pad info of forward_images / forward_batch([B,6] offsets)
-        self._raw_host = self._raw_dev = None           # raw image staging of forward_images (grown on demand)
+        self.raw = RawStager(dev)                       # raw image staging of forward_images
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -250,28 +250,31 @@ class BEV(torch.nn.Module):
             row = src[0].numel() * src.element_size()
             _lib.check(lib.b200romp_gather_rows(_ptr(src), row, _ptr(b["sel"]), _ptr(b["count2"]), cap, _ptr(dst), sp), "gather_rows")
 
-    def collect(self, to_numpy=True):
+    def _counts(self, detected, kept):
+        """The host sync of a result: (persons detected, persons kept by the filters) from two device counters."""
         with torch.cuda.stream(self.stream):
-            self.count_host[0:1].copy_(self.buf["count"], non_blocking=True)
-            self.count_host[1:2].copy_(self.buf["count2"], non_blocking=True)
+            self.count_host[0:1].copy_(detected, non_blocking=True)
+            self.count_host[1:2].copy_(kept, non_blocking=True)
         self.stream.synchronize()
-        n_det, n = int(self.count_host[0]), int(self.count_host[1])
-        if n_det == 0:
-            return None
-        if not self.calc_smpl:
-            b = self.buf
-            out = {"smpl_thetas": b["thetas"][:n_det], "smpl_betas": b["betas"][:n_det], "cam": b["cam"][:n_det],
-                   "cam_trans": b["cam_trans"][:n_det], "params_pred": b["params_pred"][:n_det],
-                   "center_confs": b["conf"][:n_det], "pred_batch_ids": b["batch_ids"][:n_det]}
-        else:
-            o = self.out
-            out = {"smpl_thetas": o["thetas"][:n], "smpl_betas": o["betas"][:n], "cam": o["cam"][:n], "cam_trans": o["cam_trans"][:n],
-                   "params_pred": o["params_pred"][:n], "center_confs": o["conf"][:n], "pred_batch_ids": o["batch_ids"][:n],
-                   "verts": o["verts"][:n], "joints": o["joints"][:n], "pj2d_org": o["pj2d_org"][:n]}
+        return int(self.count_host[0]), int(self.count_host[1])
+
+    def _result(self, src, n, batch_ids, to_numpy):
+        """The output dict (result_keys, plus the SMPL outputs) from the first n rows of the buffers ``src``."""
+        out = {"smpl_thetas": src["thetas"][:n], "smpl_betas": src["betas"][:n], "cam": src["cam"][:n], "cam_trans": src["cam_trans"][:n],
+               "params_pred": src["params_pred"][:n], "center_confs": src["conf"][:n], "pred_batch_ids": batch_ids}
+        if self.calc_smpl:
+            out.update(verts=src["verts"][:n], joints=src["joints"][:n], pj2d_org=src["pj2d_org"][:n])
         if to_numpy:
             with torch.cuda.stream(self.stream):
                 out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
         return out
+
+    def collect(self, to_numpy=True):
+        n_det, n = self._counts(self.buf["count"], self.buf["count2"])
+        if n_det == 0:
+            return None
+        src, n = (self.out, n) if self.calc_smpl else (self.buf, n_det)
+        return self._result(src, n, src["batch_ids"][:n], to_numpy)
 
     @torch.no_grad()
     def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0):
@@ -281,25 +284,13 @@ class BEV(torch.nn.Module):
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         B = frames.shape[0]
-        # device-resident inputs come from the caller's current stream: order self.stream after it (no host sync)
-        cur = torch.cuda.current_stream(self.tdevice)
-        for t in (frames, center3d_override, offsets):
-            if isinstance(t, torch.Tensor) and t.is_cuda:
-                if cur != self.stream:
-                    self.stream.wait_stream(cur)
-                t.record_stream(self.stream)
-        key = (frames.dtype, B)
-        if key not in self._staging:                  # stable pointer -> one cached CUDA graph per (dtype, B)
-            self._staging[key] = torch.empty((B, 512, 512, 3), dtype=frames.dtype, device=self.tdevice)
-        fd = self._staging[key]
+        after_producers(self.stream, self.tdevice, frames, center3d_override, offsets)
+        fd = frame_buffer(self._frames, frames.dtype, B, self.tdevice)
         with torch.cuda.stream(self.stream):
             fd.copy_(frames, non_blocking=True)
-            if offsets is not None and np.ndim(offsets) == 2:
-                assert tuple(np.shape(offsets)) == (B, 6), "per-frame offsets must be [B,6]"
-                offsets = self.pad_table[:B].copy_(torch.as_tensor(np.asarray(offsets, np.float32) if not isinstance(offsets, torch.Tensor)
-                                                                   else offsets.float()))
+            offsets = frame_offsets(offsets, self.pad_table, B)
             self.run_model(fd, center3d_override)
-            self.run_post(B, offsets if offsets is not None else [0, 512, 0, 512, 512, 512], img_max_side)
+            self.run_post(B, offsets, img_max_side)
         return self.collect(to_numpy)
 
     @torch.no_grad()
@@ -323,9 +314,7 @@ class BEV(torch.nn.Module):
                 normal.append(i)
         if center3d_override is not None:
             assert center3d_override.is_cuda and center3d_override.shape[0] == len(normal)
-            if torch.cuda.current_stream(self.tdevice) != self.stream:
-                self.stream.wait_stream(torch.cuda.current_stream(self.tdevice))
-            center3d_override.record_stream(self.stream)
+            after_producers(self.stream, self.tdevice, center3d_override)
         for c0 in range(0, len(normal), self.max_batch):
             idx = normal[c0:c0 + self.max_batch]
             for i, r in zip(idx, self._forward_chunk([imgs[i] for i in idx], to_numpy,
@@ -336,26 +325,14 @@ class BEV(torch.nn.Module):
     def _forward_chunk(self, imgs, to_numpy, center3d_override):
         """One chunk of normal images: staging + one H2D, batched preprocessing, model, per-frame post; one host sync."""
         B = len(imgs)
-        offs, total = staging_layout(imgs)
-        if total and (self._raw_host is None or self._raw_host.numel() < total):
-            self.stream.synchronize()                       # the previous chunk's preprocessing no longer reads the old buffers
-            self._raw_host = torch.empty(max(total, 1 << 24), dtype=torch.uint8).pin_memory()
-            self._raw_dev = torch.empty(self._raw_host.numel(), dtype=torch.uint8, device=self.tdevice)
-        stage_host_images(imgs, offs, self._raw_host)        # the previous chunk ended in a host sync: the buffer is free
-        cur = torch.cuda.current_stream(self.tdevice)
-        for t in imgs:
-            if t.is_cuda:
-                if cur != self.stream:
-                    self.stream.wait_stream(cur)
-                t.record_stream(self.stream)
-        key = (torch.uint8, B)
-        if key not in self._staging:
-            self._staging[key] = torch.empty((B, 512, 512, 3), dtype=torch.uint8, device=self.tdevice)
-        fd = self._staging[key]
+        # the previous chunk ended in a host sync: the pinned buffer is free, and self.stream is the last reader of both
+        offs, total = self.raw.stage(imgs, replace_after=self.stream)
+        after_producers(self.stream, self.tdevice, *imgs)
+        fd = frame_buffer(self._frames, torch.uint8, B, self.tdevice)
         with torch.cuda.stream(self.stream):
             if total:
-                self._raw_dev[:total].copy_(self._raw_host[:total], non_blocking=True)
-            preprocess_bgr_batch(self.lib, imgs, offs, self._raw_dev, fd, self.pad_table, self.stream.cuda_stream)
+                self.raw.upload(total)
+            preprocess_bgr_batch(self.lib, imgs, offs, self.raw.dev, fd, self.pad_table, self.stream.cuda_stream)
             self.run_model(fd, center3d_override)
             self.run_post(B, self.pad_table[:B])
         out = self.collect(to_numpy)
@@ -363,17 +340,11 @@ class BEV(torch.nn.Module):
             return [None] * B
         n_det = int(self.count_host[0])
         detected = set(self.buf["batch_ids"][:n_det].cpu().tolist())       # frames with a detection (before the filters)
-        ids = out["pred_batch_ids"]
-        ids = ids.cpu().numpy() if isinstance(ids, torch.Tensor) else ids
-        res = []
-        for i, (a, b) in enumerate(split_by_frame(ids, B)):
-            if i not in detected:                          # forward_batch on this frame alone returns None
-                res.append(None)
-                continue
-            r = {k: (np.array(v[a:b]) if to_numpy else v[a:b].clone()) for k, v in out.items()}
-            r["pred_batch_ids"] = np.zeros(b - a, np.int64) if to_numpy else torch.zeros(b - a, dtype=torch.int64, device=self.tdevice)
-            res.append(r)
-        return res
+        res = split_by_frame(out, B, to_numpy)
+        for i, r in enumerate(res):
+            n = len(r["cam"])
+            r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
+        return [r if i in detected else None for i, r in enumerate(res)]      # an undetected frame alone returns None
 
     def _long_buffers(self, rows):
         """Image-level accumulation rows of the long-image mode (grown on demand, kept for the next image)."""
@@ -404,24 +375,17 @@ class BEV(torch.nn.Module):
         center3d_override: optional device [K,64,128,128] replacing the crops' 3-D centre maps (tests, measurement)."""
         if not self.calc_smpl:
             raise ValueError("the long-image mode needs SMPL (bev/main.py:203): calc_smpl must be on for images with w/h >= 2")
-        img = torch.from_numpy(np.ascontiguousarray(full_image)) if isinstance(full_image, np.ndarray) else full_image
-        assert img.dtype == torch.uint8 and img.dim() == 3 and img.shape[2] == 3, "image must be HxWx3 uint8 (BGR)"
+        img = image_tensor(full_image)
         s = self.settings
         h, w = int(img.shape[0]), int(img.shape[1])
         pad_length, boxes, pad_info = long_image_plan(h, w, s.overlap_ratio)
         K, B = len(boxes), self.max_batch
         if center3d_override is not None:
             assert center3d_override.is_cuda and tuple(center3d_override.shape) == (K, 64, 128, 128)
-            cur = torch.cuda.current_stream(self.tdevice)
-            if cur != self.stream:
-                self.stream.wait_stream(cur)
-            center3d_override.record_stream(self.stream)
+            after_producers(self.stream, self.tdevice, center3d_override)
         lb = self._long_buffers(K * MAX_PERSON)
         tab = torch.from_numpy(long_image_crop_table(boxes, pad_length, h, w, float(s.nms_thresh))).pin_memory()
-        key = (torch.uint8, B)
-        if key not in self._staging:
-            self._staging[key] = torch.empty((B, 512, 512, 3), dtype=torch.uint8, device=self.tdevice)
-        frames = self._staging[key]
+        frames = frame_buffer(self._frames, torch.uint8, B, self.tdevice)
         with torch.cuda.stream(self.stream):
             padded = self.pad_long_image(img, pad_length)
             tab_dev = tab.to(self.tdevice, non_blocking=True)
@@ -480,23 +444,11 @@ class BEV(torch.nn.Module):
 
     def _collect_long(self, to_numpy=True):
         lb = self._long
-        with torch.cuda.stream(self.stream):
-            self.count_host[0:1].copy_(lb["count"][1:2], non_blocking=True)            # persons detected in any crop
-            self.count_host[1:2].copy_(lb["count2"], non_blocking=True)
-        self.stream.synchronize()
-        n_det, n = int(self.count_host[0]), int(self.count_host[1])
+        n_det, n = self._counts(lb["count"][1:2], lb["count2"])      # persons detected in any crop, persons kept
         if n_det == 0:                        # the reference raises KeyError here (main.py:253); INTEGRATION.md, Deviations
             print("No person detected!")
             return None
-        o = lb["out"]
-        out = {"smpl_thetas": o["thetas"][:n], "smpl_betas": o["betas"][:n], "cam": o["cam"][:n], "cam_trans": o["cam_trans"][:n],
-               "params_pred": o["params_pred"][:n], "center_confs": o["conf"][:n],
-               "pred_batch_ids": torch.zeros(n, dtype=torch.int64, device=self.tdevice),
-               "verts": o["verts"][:n], "joints": o["joints"][:n], "pj2d_org": o["pj2d_org"][:n]}
-        if to_numpy:
-            with torch.cuda.stream(self.stream):
-                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
-        return out
+        return self._result(lb["out"], n, torch.zeros(n, dtype=torch.int64, device=self.tdevice), to_numpy)
 
     @torch.no_grad()
     def forward(self, image, signal_ID=0, **kwargs):

@@ -22,6 +22,7 @@ import torch
 
 from . import _lib, graph
 from ._lib import BF16, F32, U8
+from .staging import FULL_FRAME, RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, split_by_frame
 
 MAX_PERSON = 64          # CenterMap.max_person, post_parser.py:11
 N_PARAMS = 145           # 3 cam + 22*6 rot6d + 10 betas, model.py:429
@@ -138,53 +139,6 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
-def image_tensor(image):
-    """HxWx3 uint8 BGR image (numpy, host or device tensor) -> a torch tensor the batched preprocessing can read: host
-    images as they are (they are copied into pinned staging), device images in place when their rows are packed BGR
-    pixels (any row stride >= 3w), else a contiguous copy."""
-    t = torch.from_numpy(np.ascontiguousarray(image)) if isinstance(image, np.ndarray) else image
-    assert isinstance(t, torch.Tensor) and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3, "image must be HxWx3 uint8 (BGR)"
-    assert t.shape[0] > 0 and t.shape[1] > 0, "empty image"
-    if t.is_cuda and not (t.stride(2) == 1 and t.stride(1) == 3 and t.stride(0) >= 3 * t.shape[1]):
-        t = t.contiguous()
-    return t
-
-
-def staging_layout(images):
-    """Byte offset of every host image inside one staging buffer (256-byte aligned; None for device images) and its size."""
-    offs, total = [], 0
-    for t in images:
-        offs.append(None if t.is_cuda else total)
-        if not t.is_cuda:
-            total += (t.numel() + 255) // 256 * 256
-    return offs, total
-
-
-def stage_host_images(images, offs, raw_host):
-    """Copy the host images into the pinned staging buffer (torch's copy_ splits each large copy over its CPU threads)."""
-    for t, o in zip(images, offs):
-        if o is not None:
-            raw_host[o:o + t.numel()].view(t.shape).copy_(t)
-
-
-def preprocess_bgr_batch(lib, images, offs, raw_dev, out, pad_table, stream):
-    """b200romp_preprocess_bgr_batch: images[i] (device tensor, or host tensor staged at raw_dev[offs[i]:]) -> out[i]
-    [512,512,3] uint8 RGB on the device, pad info into the device table pad_table [n,6] (may be None)."""
-    n = len(images)
-    ptrs = [t.data_ptr() if o is None else raw_dev.data_ptr() + o for t, o in zip(images, offs)]
-    strides = [t.stride(0) if o is None else 3 * int(t.shape[1]) for t, o in zip(images, offs)]
-    _lib.check(lib.b200romp_preprocess_bgr_batch((C.c_void_p * n)(*ptrs), (C.c_int * n)(*[int(t.shape[0]) for t in images]),
-                                                 (C.c_int * n)(*[int(t.shape[1]) for t in images]), (C.c_int * n)(*strides), n, 512,
-                                                 _ptr(out), None if pad_table is None else _ptr(pad_table), C.c_void_p(stream)),
-               "preprocess_bgr_batch")
-
-
-def split_by_frame(batch_ids, n_frames):
-    """Rows of a batch result grouped by frame (rows come in frame order): [(start, end)] per frame."""
-    b = np.searchsorted(np.asarray(batch_ids), np.arange(n_frames + 1))
-    return list(zip(b[:-1].tolist(), b[1:].tolist()))
-
-
 class SMPLParser:
     """Seam S3 (post_parser.SMPL_parser, post_parser.py:116-125) on libb200romp's fused SMPL kernels."""
 
@@ -232,7 +186,7 @@ class MapsModule(torch.nn.Module):
 
     def forward(self, frames):
         o = self._owner
-        o._after_producers(frames)
+        after_producers(o.stream, o.tdevice, frames)
         with torch.cuda.stream(o.stream):
             c, p = o.run_maps(frames.contiguous())
         torch.cuda.current_stream(o.tdevice).wait_stream(o.stream)
@@ -313,9 +267,8 @@ class ROMP(torch.nn.Module):
                 d.update(verts=z(cap, 6890, 3), joints=z(cap, 71, 3))
             self.slots.append(dict(dev=d, host=None, count_host=torch.zeros(1, dtype=torch.int32).pin_memory(),
                                    done=torch.cuda.Event(), frames={}, h2d=torch.cuda.Event(),
-                                   pad=z(B, 6), raw_host=None, raw_dev=None))   # per-frame pad info, raw image staging
+                                   pad=z(B, 6), raw=RawStager(dev)))   # per-frame pad info, raw image staging
         self._slot = 0
-        self._raw_host = self._raw_dev = None
         self.copy_stream = torch.cuda.Stream(device=dev)
         self.d2h_stream = torch.cuda.Stream(device=dev)
 
@@ -365,7 +318,7 @@ class ROMP(torch.nn.Module):
         cnt = b["count"] if count_on_device else None
         cp = None if cnt is None else _ptr(cnt)
         per_frame = isinstance(offsets, torch.Tensor) and offsets.dim() == 2
-        off = (C.c_float * 6)(*[float(v) for v in ([0, 512, 0, 512, 512, 512] if per_frame else offsets)])
+        off = (C.c_float * 6)(*[float(v) for v in (FULL_FRAME if per_frame else offsets)])
         if self.calc_smpl:
             self.smpl.forward(b["betas"], b["thetas"], cap, cnt, self.settings.root_align, sh["smpl_ws"],
                               b["verts"], b["joints"], self.stream.cuda_stream)
@@ -432,24 +385,11 @@ class ROMP(torch.nn.Module):
         return {k: v.numpy() for k, v in self._views(host, n).items()}
 
     # ------------------------------------------------------------------------------------------
-    def _after_producers(self, *tensors):
-        """Device-resident inputs were produced on the caller's current stream; our kernels run on self.stream.  Order
-        them (no host sync) and keep the allocator from recycling the inputs while self.stream still reads them."""
-        cur = torch.cuda.current_stream(self.tdevice)
-        waited = False
-        for t in tensors:
-            if isinstance(t, torch.Tensor) and t.is_cuda:
-                if not waited and cur != self.stream:
-                    self.stream.wait_stream(cur)
-                    waited = True
-                t.record_stream(self.stream)
-
-    def _staging(self, slot, dtype, B):
-        """persistent device frame buffer of a slot: a stable pointer keeps the conv graph's CUDA-graph cache at one entry"""
-        key = (dtype, B)
-        if key not in slot["frames"]:
-            slot["frames"][key] = torch.empty((B, 512, 512, 3), dtype=dtype, device=self.tdevice)
-        return slot["frames"][key]
+    def _apply_cam_trans(self, out):
+        """``--cam_trans pnp``: the reference's default estimator replaces the device's closed form, on the host."""
+        if getattr(self.settings, "cam_trans", "lsq") == "pnp" and self.calc_smpl:
+            out["cam_trans"] = estimate_translation_pnp(out["joints"], out["cam"])
+        return out
 
     @torch.no_grad()
     def forward_batch(self, frames, offsets=None, to_numpy=True, center_override=None, own=True):
@@ -460,27 +400,10 @@ class ROMP(torch.nn.Module):
         Device-resident ``frames`` / ``center_override`` may come straight from a producer on the caller's current
         stream.  ``own=True`` (default) returns arrays that own their memory; ``own=False`` returns views of the pinned
         read-back mirrors, valid until the second-next batch."""
-        if isinstance(frames, np.ndarray):
-            frames = torch.from_numpy(frames)
-        B = frames.shape[0]
-        self._slot ^= 1
-        slot = self.slots[self._slot]
-        self._after_producers(frames, center_override, offsets)
-        with torch.cuda.stream(self.stream):
-            fd = self._staging(slot, frames.dtype, B)
-            fd.copy_(frames, non_blocking=True)
-            if offsets is not None and np.ndim(offsets) == 2:
-                assert tuple(np.shape(offsets)) == (B, 6), "per-frame offsets must be [B,6]"
-                offsets = slot["pad"][:B].copy_(torch.as_tensor(np.asarray(offsets, np.float32) if not isinstance(offsets, torch.Tensor)
-                                                                else offsets.float()))
-            self.run_maps(fd)
-            self.run_post(B, offsets if offsets is not None else [0, 512, 0, 512, 512, 512], center_override)
-            slot["done"].record(self.stream)
-        out = self.collect(to_numpy)
+        after_producers(self.stream, self.tdevice, center_override, offsets)
+        out = self._read_back(self._submit_frames(frames, offsets, center_override), to_numpy)
         if out is not None and to_numpy and own:
-            out = {k: np.array(v) for k, v in out.items()}
-            if getattr(self.settings, "cam_trans", "lsq") == "pnp" and self.calc_smpl:
-                out["cam_trans"] = estimate_translation_pnp(out["joints"], out["cam"])
+            out = self._apply_cam_trans({k: np.array(v) for k, v in out.items()})
         return out
 
     @torch.no_grad()
@@ -494,36 +417,10 @@ class ROMP(torch.nn.Module):
         ``frame_offset``; each batch's records are then packed and all-gathered on the gather's side stream right after
         its kernels, and the generator yields ``(own_result, gather_handle)`` pairs (own shard read back to this rank's
         host; ``gather.result(handle)`` gives every rank's persons on the device)."""
-        off = offsets if offsets is not None else [0, 512, 0, 512, 512, 512]
         pending = None
-        self._after_producers(center_override)
+        after_producers(self.stream, self.tdevice, center_override, offsets)
         for frames in batches:
-            if isinstance(frames, np.ndarray):
-                frames = torch.from_numpy(frames)
-            B = frames.shape[0]
-            self._slot ^= 1
-            slot = self.slots[self._slot]
-            fd = self._staging(slot, frames.dtype, B)
-            if frames.is_cuda:
-                self.copy_stream.wait_stream(torch.cuda.current_stream(self.tdevice))
-                frames.record_stream(self.copy_stream)
-            with torch.cuda.stream(self.copy_stream):
-                self.copy_stream.wait_event(slot["done"])          # the slot's previous kernels no longer read fd
-                fd.copy_(frames, non_blocking=True)
-                slot["h2d"].record(self.copy_stream)
-            with torch.cuda.stream(self.stream):
-                self.stream.wait_event(slot["h2d"])
-                if slot.get("packed") is not None:
-                    self.stream.wait_event(slot["packed"])          # the gather's pack kernel has read the slot's previous results
-                self.run_maps(fd)
-                self.run_post(B, off, center_override, slot)
-                slot["done"].record(self.stream)
-                if gather is not None:
-                    fields, count = self.record_fields(slot)
-                    slot["gather"] = gather.submit(fields, count, frame_offset)
-                    slot["packed"] = slot["gather"]["packed"]
-            if not frames.is_cuda:
-                slot["h2d"].synchronize()     # the caller may refill its (single) host buffer as soon as we yield / pull the next batch
+            slot = self._submit_frames(frames, offsets, center_override, gather, frame_offset)
             if pending is not None:
                 res = self._read_back(pending, to_numpy)
                 yield (res, pending["gather"]) if gather is not None else res
@@ -531,6 +428,35 @@ class ROMP(torch.nn.Module):
         if pending is not None:
             res = self._read_back(pending, to_numpy)
             yield (res, pending["gather"]) if gather is not None else res
+
+    def _submit_frames(self, frames, offsets, center_override, gather=None, frame_offset=0):
+        """One batch of frames into the next slot: H2D into the slot's frame buffer on the copy stream, the kernels on
+        self.stream.  Returns once host frames have been copied, so the caller may refill their buffer."""
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(frames)
+        B = frames.shape[0]
+        self._slot ^= 1
+        slot = self.slots[self._slot]
+        fd = frame_buffer(slot["frames"], frames.dtype, B, self.tdevice)
+        after_producers(self.copy_stream, self.tdevice, frames)
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_event(slot["done"])          # the slot's previous kernels no longer read fd
+            fd.copy_(frames, non_blocking=True)
+            slot["h2d"].record(self.copy_stream)
+        with torch.cuda.stream(self.stream):
+            self.stream.wait_event(slot["h2d"])
+            if slot.get("packed") is not None:
+                self.stream.wait_event(slot["packed"])          # the gather's pack kernel has read the slot's previous results
+            self.run_maps(fd)
+            self.run_post(B, frame_offsets(offsets, slot["pad"], B), center_override, slot)
+            slot["done"].record(self.stream)
+            if gather is not None:
+                fields, count = self.record_fields(slot)
+                slot["gather"] = gather.submit(fields, count, frame_offset)
+                slot["packed"] = slot["gather"]["packed"]
+        if not frames.is_cuda:
+            slot["h2d"].synchronize()     # the caller may refill its (single) host buffer as soon as we yield / pull the next batch
+        return slot
 
     def _read_back(self, slot, to_numpy=True):
         self.d2h_stream.wait_event(slot["done"])
@@ -554,7 +480,7 @@ class ROMP(torch.nn.Module):
         every list, entry k to the k-th image of the list."""
         if self.temporal is not None:
             raise NotImplementedError("--temporal_optimize smooths one image sequence: call forward() per frame")
-        self._after_producers(center_override)
+        after_producers(self.stream, self.tdevice, center_override)
 
         def chunks():
             for images in batches:
@@ -577,30 +503,35 @@ class ROMP(torch.nn.Module):
         if pending is not None:
             yield self._finish_images(*pending, to_numpy)
 
-    def _submit_images(self, imgs, center_override):
-        B = len(imgs)
+    def _upload(self, slot, imgs):
+        """Host images into the slot's pinned staging buffer and to the device with one H2D on the copy stream; self.stream
+        is ordered after that copy and after the producers of device images.  Returns each image's byte offset in
+        slot["raw"].dev (None: a device image, read in place)."""
+        raw = slot["raw"]
+        offs, total = raw.stage(imgs, replace_after=slot["done"], reuse_after=slot["h2d"])
+        if total:
+            with torch.cuda.stream(self.copy_stream):
+                self.copy_stream.wait_event(slot["done"])  # the slot's previous preprocessing no longer reads raw.dev
+                raw.upload(total)
+                slot["h2d"].record(self.copy_stream)
+            self.stream.wait_event(slot["h2d"])
+        after_producers(self.stream, self.tdevice, *imgs)
+        return offs
+
+    def _preprocess_images(self, imgs):
+        """Raw images into the next slot's frames and pad table: one preprocessing kernel on self.stream."""
         self._slot ^= 1
         slot = self.slots[self._slot]
-        fd = self._staging(slot, torch.uint8, B)
-        offs, total = staging_layout(imgs)
-        if total:
-            if slot["raw_host"] is None or slot["raw_host"].numel() < total:
-                slot["done"].synchronize()                 # the slot's previous kernels no longer read the old buffers
-                n = max(total, 1 << 24)
-                slot["raw_host"] = torch.empty(n, dtype=torch.uint8).pin_memory()
-                slot["raw_dev"] = torch.empty(n, dtype=torch.uint8, device=self.tdevice)
-            else:
-                slot["h2d"].synchronize()                  # the slot's previous H2D has left its pinned buffer
-            stage_host_images(imgs, offs, slot["raw_host"])
-            with torch.cuda.stream(self.copy_stream):
-                self.copy_stream.wait_event(slot["done"])  # the slot's previous preprocessing no longer reads raw_dev
-                slot["raw_dev"][:total].copy_(slot["raw_host"][:total], non_blocking=True)
-                slot["h2d"].record(self.copy_stream)
-        self._after_producers(*[t for t in imgs if t.is_cuda])
+        fd = frame_buffer(slot["frames"], torch.uint8, len(imgs), self.tdevice)
+        offs = self._upload(slot, imgs)
         with torch.cuda.stream(self.stream):
-            if total:
-                self.stream.wait_event(slot["h2d"])
-            preprocess_bgr_batch(self.lib, imgs, offs, slot["raw_dev"], fd, slot["pad"], self.stream.cuda_stream)
+            preprocess_bgr_batch(self.lib, imgs, offs, slot["raw"].dev, fd, slot["pad"], self.stream.cuda_stream)
+        return slot, fd
+
+    def _submit_images(self, imgs, center_override):
+        B = len(imgs)
+        slot, fd = self._preprocess_images(imgs)
+        with torch.cuda.stream(self.stream):
             self.run_maps(fd)
             self.run_post(B, slot["pad"][:B], center_override, slot)
             slot["done"].record(self.stream)
@@ -610,76 +541,47 @@ class ROMP(torch.nn.Module):
         """Read back one chunk and scatter its persons to res[c0:c0+B]; returns res once its last chunk is in."""
         out = None if slot is None else self._read_back(slot, to_numpy)
         if out is not None:
-            ids = out["pred_batch_ids"]
-            ids = ids.cpu().numpy() if isinstance(ids, torch.Tensor) else ids
-            pnp = to_numpy and self.calc_smpl and getattr(self.settings, "cam_trans", "lsq") == "pnp"
-            for i, (a, b) in enumerate(split_by_frame(ids, B)):
-                if a == b:
-                    continue
-                r = {k: (np.array(v[a:b]) if to_numpy else v[a:b].clone()) for k, v in out.items() if k != "pred_batch_ids"}
-                if pnp:
-                    r["cam_trans"] = estimate_translation_pnp(r["joints"], r["cam"])
-                res[c0 + i] = r
+            for i, r in enumerate(split_by_frame(out, B, to_numpy)):
+                if len(r["cam"]):
+                    r.pop("pred_batch_ids")
+                    res[c0 + i] = self._apply_cam_trans(r) if to_numpy else r
         return res if last else None
 
     @torch.no_grad()
     def preprocess(self, image, out=None):
         """img_preprocess (utils.py:26-30) on the GPU: raw HxWx3 uint8 BGR image (numpy / host tensor / device tensor) ->
         ``out`` [512,512,3] uint8 RGB on the device (allocated when None) + pad info [top,bottom,left,right,h,w].
-        One kernel (b200romp_preprocess_bgr) on self.stream; the only host work is the H2D copy of the raw image."""
-        img = torch.from_numpy(np.ascontiguousarray(image)) if isinstance(image, np.ndarray) else image
-        assert img.dtype == torch.uint8 and img.dim() == 3 and img.shape[2] == 3, "image must be HxWx3 uint8 (BGR)"
+        One kernel (b200romp_preprocess_bgr) on self.stream; a host image is staged through the current slot."""
+        img = image_tensor(image)
         h, w = int(img.shape[0]), int(img.shape[1])
         if out is None:
             out = torch.empty((512, 512, 3), dtype=torch.uint8, device=self.tdevice)
-        if img.is_cuda:
-            self._after_producers(img)
-            raw = img.contiguous()
-        else:
-            n = img.numel()
-            if self._raw_host is None or self._raw_host.numel() < n:
-                self._raw_host = torch.empty(max(n, 1 << 22), dtype=torch.uint8).pin_memory()
-                self._raw_dev = torch.empty(self._raw_host.numel(), dtype=torch.uint8, device=self.tdevice)
-            self.stream.synchronize()                       # the previous image's H2D has left the pinned staging buffer
-            self._raw_host[:n].copy_(img.reshape(-1))
-            raw = self._raw_dev[:n]
-            with torch.cuda.stream(self.stream):
-                raw.copy_(self._raw_host[:n], non_blocking=True)
+        slot = self.slots[self._slot]
+        off = self._upload(slot, [img])[0]
+        raw, stride = (img.data_ptr(), img.stride(0)) if off is None else (slot["raw"].dev.data_ptr() + off, 3 * w)
         pad = (C.c_float * 6)()
-        _lib.check(self.lib.b200romp_preprocess_bgr(_ptr(raw), h, w, 3 * w, 512, _ptr(out), pad,
+        _lib.check(self.lib.b200romp_preprocess_bgr(C.c_void_p(raw), h, w, stride, 512, _ptr(out), pad,
                                                     C.c_void_p(self.stream.cuda_stream)), "preprocess_bgr")
+        slot["done"].record(self.stream)                  # the slot's staging buffer is read until here
         return out, np.array(list(pad), dtype=np.float32)
 
     @torch.no_grad()
     def forward(self, image, signal_ID=0, **kwargs):
         """image: HxWx3 uint8 BGR (cv2.imread).  main.py:160-176; preprocessing, model, parse, SMPL and projection all run
         on the GPU - OpenCV is not involved."""
-        self._slot ^= 1
-        slot = self.slots[self._slot]
-        fd = self._staging(slot, torch.uint8, 1)
-        _, pad_info = self.preprocess(image, out=fd[0])
         if self.temporal is not None:
-            return self._forward_temporal(fd, pad_info, slot, signal_ID)
-        with torch.cuda.stream(self.stream):
-            self.run_maps(fd)
-            self.run_post(1, pad_info)
-            slot["done"].record(self.stream)
-        out = self.collect(True)
+            return self._forward_temporal(image, signal_ID)
+        out = self.forward_images([image])[0]
         if out is None:
             print("None person detected")                                       # post_parser.py:139
-            return None
-        out.pop("pred_batch_ids")
-        out = {k: np.array(v) for k, v in out.items()}                           # arrays own their memory like the reference's
-        if getattr(self.settings, "cam_trans", "lsq") == "pnp" and self.calc_smpl:
-            out["cam_trans"] = estimate_translation_pnp(out["joints"], out["cam"])
         return out
 
-
     @torch.no_grad()
-    def _forward_temporal(self, fd, pad_info, slot, signal_ID):
+    def _forward_temporal(self, image, signal_ID):
         """forward() with --temporal_optimize (main.py:164-165 -> temporal_optimization :127-157): parse, associate the
         detections with tracks on the host (needs the cams: one small D2H, like the reference), One-Euro smoothing of
         thetas / betas / cam on the device, then SMPL + projection on the smoothed parameters."""
+        slot, fd = self._preprocess_images([image_tensor(image)])
         b, lib, sp = slot["dev"], self.lib, C.c_void_p(self.stream.cuda_stream)
         with torch.cuda.stream(self.stream):
             self.run_maps(fd)
@@ -707,7 +609,7 @@ class ROMP(torch.nn.Module):
                 for key in ("thetas", "betas", "cam"):
                     b[key][0].copy_(b[key][k].clone())
                 n_smpl = 1
-            self.run_smpl_project(n_smpl, pad_info, slot, count_on_device=False)
+            self.run_smpl_project(n_smpl, slot["pad"][:1], slot, count_on_device=False)
             slot["done"].record(self.stream)
             host = self._host(slot)
             for key, v in b.items():

@@ -32,7 +32,7 @@ sys.path.insert(0, ROOT)
 from oracle import preproc_oracle as P  # noqa: E402
 from oracle import romp_oracle as O  # noqa: E402
 from romp_b200 import ROMP, _lib, romp_settings, synth  # noqa: E402
-from romp_b200.main import image_tensor, preprocess_bgr_batch, stage_host_images, staging_layout  # noqa: E402
+from romp_b200.staging import image_tensor, preprocess_bgr_batch, stage_host_images, staging_layout  # noqa: E402
 
 SHAPES = [(1080, 1920), (720, 1280), (1920, 1080), (480, 640)]
 
