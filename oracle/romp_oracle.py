@@ -316,35 +316,44 @@ def parsing_outputs(center_maps, params_maps, thresh=0.25):
 # ----------------------------------------------------------------------------------------------
 # a13-a16: SMPL forward  (simple_romp/romp/smpl.py:24-35,62-290; SURVEY appendix D)
 # ----------------------------------------------------------------------------------------------
-def batch_rodrigues(rv):
-    """smpl.py:191-222.  NB eps is added to every component before the norm (:206)."""
+def batch_rodrigues(rv, dtype=torch.float32, device="cpu"):
+    """smpl.py:191-222.  NB eps is added to every component before the norm (:206).  ``dtype`` / ``device``: where and in
+    which precision to compute (the defaults are the reference's CPU fp32 arithmetic)."""
+    rv = _t(rv).to(device=device, dtype=dtype)
     angle = torch.norm(rv + 1e-8, dim=1, keepdim=True)
     d = rv / angle
     c, s = torch.cos(angle)[:, :, None], torch.sin(angle)[:, :, None]
     rx, ry, rz = d[:, 0:1], d[:, 1:2], d[:, 2:3]
     z = torch.zeros_like(rx)
     K = torch.cat([z, -rz, ry, rz, z, -rx, -ry, rx, z], 1).view(-1, 3, 3)
-    return torch.eye(3).unsqueeze(0) + s * K + (1 - c) * torch.bmm(K, K)
+    return torch.eye(3, dtype=dtype, device=device).unsqueeze(0) + s * K + (1 - c) * torch.bmm(K, K)
 
 
-def smpl_forward(pack, betas, thetas, root_align=False, shape_key="shapedirs"):
+def smpl_forward(pack, betas, thetas, root_align=False, shape_key="shapedirs", dtype=torch.float32, device="cpu",
+                 stages=False):
     """SMPL.forward + lbs + batch_rigid_transform + VertexJointSelector (smpl.py:62-108,111-188,236-290,24-35).
 
-    Returns verts [N,6890,3], joints71 [N,71,3] (24 SMPL + 21 picked verts + 9 + 17 regressed).
+    Returns verts [N,6890,3], joints71 [N,71,3] (24 SMPL + 21 picked verts + 9 + 17 regressed).  ``dtype`` / ``device``:
+    the precision and device of every operation (the defaults are the reference's CPU fp32 arithmetic).  With ``stages``
+    a third result holds the intermediate stages: "feat" [N, n_betas+207] = [betas | (R[1:]-I)], "A" [N,24,3,4] (the
+    relative transforms), "v_posed" [N,6890,3], "T" [N,6890,4,4] (the blended transforms) and "J_regressed" [N,24,3]
+    (the rest-pose joints).
     """
     pk = {k: _t(v) for k, v in pack.items()}
-    betas, thetas = _t(betas).float(), _t(thetas).float()
+    fl = lambda x: x.to(device=device, dtype=dtype)
+    betas, thetas = fl(_t(betas)), fl(_t(thetas))
     n = betas.shape[0]
-    vt, sdirs, pdirs = pk["v_template"], pk[shape_key], pk["posedirs"]
-    Jr, W, parents = pk["J_regressor"], pk["weights"], pk["kintree_table"].tolist()
+    vt, sdirs, pdirs = fl(pk["v_template"]), fl(pk[shape_key]), fl(pk["posedirs"])
+    Jr, W, parents = fl(pk["J_regressor"]), fl(pk["weights"]), pk["kintree_table"].tolist()
+    eye3 = torch.eye(3, dtype=dtype, device=device)
     v_shaped = vt.unsqueeze(0) + torch.einsum("bl,mkl->bmk", betas, sdirs)                 # :153
     J = torch.einsum("bik,ji->bjk", v_shaped, Jr)                                           # :156
-    R = batch_rodrigues(thetas.reshape(-1, 3)).view(n, 24, 3, 3)                            # :163
-    pf = (R[:, 1:] - torch.eye(3)).reshape(n, 207)                                          # :165
+    R = batch_rodrigues(thetas.reshape(-1, 3), dtype, device).view(n, 24, 3, 3)            # :163
+    pf = (R[:, 1:] - eye3).reshape(n, 207)                                                  # :165
     v_posed = v_shaped + torch.matmul(pf, pdirs).view(n, -1, 3)                             # :167-170
     rel = J.clone()
     rel[:, 1:] = J[:, 1:] - J[:, parents[1:]]                                               # :262-263
-    L = torch.zeros(n, 24, 4, 4)
+    L = torch.zeros(n, 24, 4, 4, dtype=dtype, device=device)
     L[:, :, :3, :3] = R
     L[:, :, :3, 3] = rel
     L[:, :, 3, 3] = 1.0                                                                     # :224-234
@@ -353,19 +362,22 @@ def smpl_forward(pack, betas, thetas, root_align=False, shape_key="shapedirs"):
         G.append(torch.matmul(G[parents[i]], L[:, i]))                                      # :270-275
     G = torch.stack(G, 1)
     J_posed = G[:, :, :3, 3]                                                                # :280
-    Jh = torch.cat([J, torch.zeros(n, 24, 1)], 2).unsqueeze(-1)
+    Jh = torch.cat([J, torch.zeros(n, 24, 1, dtype=dtype, device=device)], 2).unsqueeze(-1)
     A = G.clone()
     A[:, :, :, 3] = G[:, :, :, 3] - torch.matmul(G, Jh)[..., 0]                             # :285-288
     T = torch.matmul(W.unsqueeze(0).expand(n, -1, -1), A.view(n, 24, 16)).view(n, -1, 4, 4)  # :176-180
-    vh = torch.cat([v_posed, torch.ones(n, v_posed.shape[1], 1)], 2).unsqueeze(-1)
+    vh = torch.cat([v_posed, torch.ones(n, v_posed.shape[1], 1, dtype=dtype, device=device)], 2).unsqueeze(-1)
     verts = torch.matmul(T, vh)[:, :, :3, 0]                                                # :182-186
-    j21 = verts[:, pk["extra_joints_index"]]
-    j9 = torch.einsum("bik,ji->bjk", verts, pk["J_regressor_extra9"])
-    j17 = torch.einsum("bik,ji->bjk", verts, pk["J_regressor_h36m17"])
+    j21 = verts[:, pk["extra_joints_index"].to(device)]
+    j9 = torch.einsum("bik,ji->bjk", verts, fl(pk["J_regressor_extra9"]))
+    j17 = torch.einsum("bik,ji->bjk", verts, fl(pk["J_regressor_h36m17"]))
     joints = torch.cat([J_posed, j21, j9, j17], 1)                                          # :25-29
     if root_align:                                                                          # :102-106
         root = joints[:, [45, 46]].mean(1, keepdim=True)
         joints, verts = joints - root, verts - root
+    if stages:
+        feat = torch.cat([betas, pf], 1)
+        return verts, joints, {"feat": feat, "A": A[:, :, :3, :], "v_posed": v_posed, "T": T, "J_regressed": J}
     return verts, joints
 
 

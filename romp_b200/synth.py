@@ -140,13 +140,52 @@ NUM_VERTS = 6890
 NUM_FACES = 13776
 
 
-def smpl_pack(seed: int = 0, num_betas: int = 10, dense_weights: bool = False):
+SMPL_PACK_VARIANTS = ("synthetic", "real_scale", "wide_range")
+
+
+def smpl_pack(seed: int = 0, num_betas: int = 10, dense_weights: bool = False, variant: str = "synthetic"):
     """Synthetic packed SMPL with human-like magnitudes.
 
     v_template ~ a 1.7 m tall point cloud, shapedirs ~ cm scale, posedirs ~ mm-cm scale,
     skinning weights with 4 non-zeros per vertex (or dense if ``dense_weights``) that sum to 1,
     joint regressors as sparse convex combinations (stored dense like the reference).
+
+    ``variant`` changes the blend matrix and the skinning weights, seeded, after the default draw:
+      * "real_scale": shapedirs ~ N(0, 0.05) and posedirs ~ N(0, 0.02), the magnitudes of the released SMPL model;
+      * "wide_range": every shapedirs / posedirs entry and 23 of the 24 skinning weights of each vertex have magnitudes
+        log-uniform in [1e-8, 1e-1] (random signs for the blend entries); the 24th weight, at a random joint, makes the
+        row sum 1.  Entries this small leave fp16 subnormal or zero hi / lo parts in a split fp16 representation.
     """
+    if variant not in SMPL_PACK_VARIANTS:
+        raise ValueError(f"smpl_pack: unknown variant {variant!r}")
+    pack = _smpl_pack_default(seed, num_betas, dense_weights)
+    if variant == "synthetic":
+        return pack
+    key = "shapedirs" if num_betas == 10 else "smpla_shapedirs"
+    rng = np.random.RandomState(seed + 104723)
+    V = NUM_VERTS
+    if variant == "real_scale":
+        shapedirs = rng.normal(0, 0.05, size=(V, 3, num_betas)).astype(np.float32)
+        pack["posedirs"] = rng.normal(0, 0.02, size=(207, V * 3)).astype(np.float32)
+    else:
+        def log_uniform(shape, signed):
+            x = 10.0 ** rng.uniform(-8, -1, size=shape)
+            return x * rng.choice([-1.0, 1.0], size=shape) if signed else x
+
+        shapedirs = log_uniform((V, 3, num_betas), True).astype(np.float32)
+        pack["posedirs"] = log_uniform((207, V * 3), True).astype(np.float32)
+        w = log_uniform((V, 24), False)
+        big = rng.randint(0, 24, size=V)
+        w[np.arange(V), big] = 0.0
+        w[np.arange(V), big] = 1.0 - w.sum(1)
+        pack["weights"] = w.astype(np.float32)
+    pack[key] = shapedirs
+    if num_betas != 10:
+        pack["shapedirs"] = shapedirs[:, :, :10].copy()
+    return pack
+
+
+def _smpl_pack_default(seed, num_betas, dense_weights):
     rng = np.random.RandomState(seed + 7919)
     V = NUM_VERTS
     v_template = (rng.uniform(-1, 1, size=(V, 3)) * np.array([0.45, 0.85, 0.15])).astype(np.float32)
