@@ -309,6 +309,40 @@ int b200romp_one_euro_smooth(b200romp_tracks* tracks, const int* slot, int n, co
                              int betas_stride, int n_betas, float* cam, float smooth_coeff, float freq, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * BEV's video mode (-t/--temporal_optimize, simple_romp/bev/main.py:109-121,165-169,260-287): the reference's 3-D-centre
+ * ByteTrack (simple_romp/tracker/byte_tracker_3dcenter.py with kalman_filter_3dcenter.py and matching.py;
+ * Tracker(det_thresh=0.12, low_conf_det_thresh=0.05, track_buffer=60, match_thresh=300, frame_rate=30), main.py:121),
+ * the One-Euro filters keyed by (signal, track) (main.py:280-285, romp/utils.py:248-270) and cam_trans from the smoothed
+ * cam (main.py:169), as ONE kernel per batch between b200romp_bev_regress and SMPL-A.  The tracker state (fp64) and the
+ * filters live in the handle; track ids count from 1 per handle.  max_tracks (1..128) bounds the live tracks (tracked +
+ * lost), max_signals the filter sets (one per track and signal).
+ *
+ * b200romp_bev_track_step steps the tracker through the frames 0..batch-1 in order, using the regressor's rows
+ * [0, min(*d_count, capacity)) grouped by frame (batch_ids, conf, cam, cam_trans, thetas [72], betas [11],
+ * params_pred [146]); a frame with no row does not step it (main.py:159-163).  signal_slot: device int32 [batch], the
+ * filter set of each frame (0 <= slot < max_signals).  For every frame the output rows are, in the reference's order,
+ * one per activated tracked track: out_batch_ids (frame), out_track_ids (int32 id), out_det (the frame-local row of the
+ * nearest detection; two rows may share one, BT:149-159), and the gathered, smoothed thetas / betas / cam with
+ * cam_trans from the smoothed cam and the gathered params_pred / conf.  A frame can give up to 128 rows.
+ * show_largest != 0: no tracker (main.py:118-119,262-267); one row per frame with a detection, the largest cam[:,0]
+ * (first on ties), smoothed with the signal's single filter set; out_track_ids = 0.
+ * *d_out_count = total rows.  d_status: device int32 [2 + batch] = {status, tracker frame_id, rows of frame 0, ...,
+ * rows of frame batch-1}; status 1 = the track table is full, 2 = more than out_capacity rows.  A nonzero status leaves the batch unfinished and every later step does nothing
+ * until b200romp_bev_tracker_reset(-1); the caller raises on it after its sync. */
+typedef struct b200romp_bev_tracker b200romp_bev_tracker;
+b200romp_bev_tracker* b200romp_bev_tracker_create(int device, int max_tracks, int max_signals);
+void b200romp_bev_tracker_destroy(b200romp_bev_tracker* tracker);
+/* signal = -1: a fresh tracker (no tracks, frame_id 0, ids from 1) and fresh filters; signal >= 0: forget that
+ * signal's filters only */
+int b200romp_bev_tracker_reset(b200romp_bev_tracker* tracker, int signal, b200romp_stream stream);
+int b200romp_bev_track_step(b200romp_bev_tracker* tracker, int batch, int capacity, const int* d_count, const long long* batch_ids,
+                            const float* conf, const float* cam, const float* cam_trans, const float* thetas, const float* betas,
+                            const float* params_pred, const int* signal_slot, int show_largest, float smooth_coeff, int out_capacity,
+                            int* d_out_count, long long* out_batch_ids, int* out_track_ids, int* out_det, float* out_thetas,
+                            float* out_betas, float* out_cam, float* out_cam_trans, float* out_params_pred, float* out_conf,
+                            int* d_status, b200romp_stream stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Frame-sharded multi-GPU collection (SURVEY 8e; the reference's DataParallel bookkeeping it stands in for:
  * romp/lib/maps_utils/result_parser.py:59-64,123-124).  Packs the per-person output arrays of one rank into the
  * fixed-width record buffer that a single NCCL all-gather ships:

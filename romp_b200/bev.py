@@ -29,6 +29,8 @@ conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.
 long_conf_dict = {1: [0.12, 20, 1.5, 0.46], 2: [0.08, 20, 1.6, 0.8]}
 model_dict = {1: "BEV_ft_agora.pth", 2: "BEV.pth"}
 N_PARAMS = 146                                                       # 3 cam + 22*6 + 11 betas, bev/model.py:116
+TRACKER_MAX_TRACKS = 128                                             # live tracks (tracked + lost) of the video mode
+MAX_SIGNALS = 4                                                      # filter sets of the video mode, the oldest evicted
 
 
 def bev_settings(input_args=sys.argv[1:]):
@@ -124,8 +126,10 @@ class BEV(torch.nn.Module):
         self.settings = s = settings
         if not torch.cuda.is_available() or s.GPU < 0:
             raise RuntimeError("romp_b200.BEV needs a CUDA device (H100, sm_90a); there is no CPU fallback")
-        if getattr(s, "temporal_optimize", False) or getattr(s, "show", False) or getattr(s, "show_largest", False):
-            raise NotImplementedError("temporal smoothing / display are outside the GPU hot path (SURVEY.md section 2)")
+        if getattr(s, "show", False):
+            raise NotImplementedError("display (--show) is outside the GPU hot path (SURVEY.md section 2)")
+        self.temporal = bool(getattr(s, "temporal_optimize", False))
+        self.show_largest = self.temporal and bool(getattr(s, "show_largest", False))
         # NB the reference renders by default (render_mesh is store_false, bev/main.py:44); rendering is out of scope and
         # simply not performed here.
         self.lib = _lib.load()
@@ -157,6 +161,8 @@ class BEV(torch.nn.Module):
             self.smpla = SMPLParser(smpla_pack, self.device_index, n_betas=11, shape_key="smpla_shapedirs")   # post_parser.py:259
             self.smil = SMPLParser(smil_pack, self.device_index, n_betas=10)                                     # :258
         self._alloc(B)
+        if self.temporal:
+            self._alloc_temporal(B)
 
     def _net(self, in_dtype):
         if in_dtype not in self._nets:
@@ -191,6 +197,125 @@ class BEV(torch.nn.Module):
         self.pad_table = z(B, 6)                       # per-frame pad info of forward_images / forward_batch([B,6] offsets)
         self.raw = RawStager(dev)                       # raw image staging of forward_images
 
+    def _alloc_temporal(self, B):
+        """The video mode (bev/main.py:109-121,260-287): one tracker per instance (shared by every signal_ID), the
+        filter sets of MAX_SIGNALS signals, and row buffers for up to 2 x 64 rows per frame."""
+        dev, R = self.tdevice, 2 * B * MAX_PERSON
+        self.trk = self.lib.b200romp_bev_tracker_create(self.device_index, TRACKER_MAX_TRACKS, MAX_SIGNALS)
+        if not self.trk:
+            raise RuntimeError("b200romp_bev_tracker_create: " + self.lib.b200romp_last_error().decode())
+        self.signals = {}                              # signal_ID -> filter set, oldest first (ROMP's TemporalState)
+        z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
+        i64, i32 = torch.int64, torch.int32
+        self.tbuf = dict(count=z(1, dtype=i32), batch_ids=z(R, dtype=i64), track_ids=z(R, dtype=i32), det=z(R, dtype=i32),
+                         thetas=z(R, 72), betas=z(R, 11), cam=z(R, 3), cam_trans=z(R, 3), params_pred=z(R, N_PARAMS), conf=z(R),
+                         status=z(2 + B, dtype=i32), sig=z(B, dtype=i32), pj2d_org=z(R, 71, 2), keep=z(R, dtype=i32),
+                         sel=z(R, dtype=i32), count2=z(1, dtype=i32))
+        if self.calc_smpl:
+            self.tbuf.update(verts=z(R, 6890, 3), joints=z(R, 71, 3), verts_smil=z(R, 6890, 3), joints_smil=z(R, 71, 3),
+                             smpl_ws=z(R, self.smpla.ws_floats))
+        self.tout = {k: torch.zeros_like(self.tbuf[k]) for k in ("batch_ids", "track_ids", "conf", "params_pred", "cam", "thetas",
+                                                                "betas", "cam_trans", "pj2d_org")}
+        if self.calc_smpl:
+            self.tout.update(verts=torch.zeros_like(self.tbuf["verts"]), joints=torch.zeros_like(self.tbuf["joints"]))
+        # the batch's one read-back: detected, rows, kept rows, then the kernel's status, frame_id and rows per frame
+        self.tsync_host = torch.zeros(5 + B, dtype=torch.int32).pin_memory()
+        self.frame_id = 0                              # tracker frames so far (frames with a detection)
+        self.tsig_host = torch.zeros(B, dtype=torch.int32).pin_memory()
+
+    def _signal_slots(self, signal_IDs):
+        """filter set of every frame's signal_ID; a new signal beyond MAX_SIGNALS evicts the oldest one (its filters are
+        reset on the stream, before the batch's kernel)."""
+        if len(set(signal_IDs)) > MAX_SIGNALS:
+            raise ValueError(f"BEV video mode: at most {MAX_SIGNALS} distinct signal_IDs per batch (their filter sets are "
+                             "used by one kernel); split the batch")
+        slots = []
+        batch = set(signal_IDs)
+        for sid in signal_IDs:
+            if sid not in self.signals:
+                if len(self.signals) >= MAX_SIGNALS:                       # the oldest signal not used by this batch
+                    self.signals.pop(next(k for k in self.signals if k not in batch))
+                used = set(self.signals.values())
+                slot = next(k for k in range(MAX_SIGNALS) if k not in used)
+                _lib.check(self.lib.b200romp_bev_tracker_reset(self.trk, slot, C.c_void_p(self.stream.cuda_stream)), "tracker_reset")
+                self.signals[sid] = slot
+            slots.append(self.signals[sid])
+        return slots
+
+    def reset_temporal(self):
+        """Forget every track, id and filter (a new video); ids start again from 1."""
+        if not self.temporal:
+            raise RuntimeError("reset_temporal: this BEV instance was built without -t/--temporal_optimize")
+        _lib.check(self.lib.b200romp_bev_tracker_reset(self.trk, -1, C.c_void_p(self.stream.cuda_stream)), "tracker_reset")
+        self.signals = {}
+
+    @torch.no_grad()
+    def run_temporal(self, B, signal_IDs):
+        """BEV.temporal_optimization (bev/main.py:165-169,260-287) of the batch's frames in order: one kernel
+        (b200romp_bev_track_step) between the regressor and SMPL-A, writing the smoothed rows to ``self.tbuf``."""
+        b, t = self.buf, self.tbuf
+        slots = self._signal_slots(signal_IDs)
+        self.tsig_host[:B].copy_(torch.tensor(slots, dtype=torch.int32))
+        t["sig"][:B].copy_(self.tsig_host[:B], non_blocking=True)
+        R = 2 * B * MAX_PERSON
+        _lib.check(self.lib.b200romp_bev_track_step(
+            self.trk, B, B * MAX_PERSON, _ptr(b["count"]), _ptr(b["batch_ids"]), _ptr(b["conf"]), _ptr(b["cam"]), _ptr(b["cam_trans"]),
+            _ptr(b["thetas"]), _ptr(b["betas"]), _ptr(b["params_pred"]), _ptr(t["sig"]), int(self.show_largest),
+            float(self.settings.smooth_coeff), R, _ptr(t["count"]), _ptr(t["batch_ids"]), _ptr(t["track_ids"]), _ptr(t["det"]),
+            _ptr(t["thetas"]), _ptr(t["betas"]), _ptr(t["cam"]), _ptr(t["cam_trans"]), _ptr(t["params_pred"]), _ptr(t["conf"]),
+            _ptr(t["status"]), C.c_void_p(self.stream.cuda_stream)), "bev_track_step")
+
+    @torch.no_grad()
+    def run_post_temporal(self, B, offsets, img_max_side=512.0):
+        """run_post on the tracker's rows (up to 2 x 64 per frame)."""
+        self.run_post(B, offsets, img_max_side, self.tbuf, self.tout, 2 * B * MAX_PERSON, self.tbuf["count"])
+
+    def _collect_temporal(self, B, to_numpy):
+        """(batch result dict, rows per frame) after the host sync; raises on a full track table."""
+        h, t = self.tsync_host, self.tbuf
+        with torch.cuda.stream(self.stream):
+            h[0:1].copy_(self.buf["count"], non_blocking=True)
+            h[1:2].copy_(t["count"], non_blocking=True)
+            h[2:3].copy_(t["count2"], non_blocking=True)
+            h[3:5 + B].copy_(t["status"][:2 + B], non_blocking=True)
+        self.stream.synchronize()
+        n_det, n_rows, n_kept, status = int(h[0]), int(h[1]), int(h[2]), int(h[3])
+        self.frame_id = int(h[4])
+        if status:
+            raise RuntimeError("BEV video mode: " + (f"more than {TRACKER_MAX_TRACKS} live tracks" if status == 1 else "too many rows")
+                               + "; call reset_temporal() before the next frame")
+        src, n = (self.tout, n_kept) if self.calc_smpl else (self.tbuf, n_rows)
+        bid = src["batch_ids"][:n]
+        out = self._result(src, n, bid, False)
+        out["_bid"] = bid
+        if not self.show_largest:
+            out["track_ids"] = src["track_ids"][:n]
+        else:                                           # bev/main.py:262-267: only thetas / betas / cam are cut to one row
+            out.update(params_pred=self.buf["params_pred"][:n_det], center_confs=self.buf["conf"][:n_det],
+                       pred_batch_ids=self.buf["batch_ids"][:n_det])
+        rows = {b for b in range(B) if int(h[5 + b])}                # frames the tracker gave rows (before the filters)
+        if to_numpy:
+            with torch.cuda.stream(self.stream):
+                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
+        return out, rows
+
+    def _split_temporal(self, out, B, rows, to_numpy):
+        """per-frame dicts of a temporal batch result (None for a frame without rows), pred_batch_ids set to 0."""
+        res = []
+        for b in range(B):
+            if b not in rows:
+                res.append(None)
+                continue
+            r = {}
+            for k, v in out.items():
+                ids = out["pred_batch_ids"] if (self.show_largest and k in ("params_pred", "center_confs", "pred_batch_ids")) else out["_bid"]
+                r[k] = v[ids == b]
+            n = len(r["pred_batch_ids"])
+            r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
+            r.pop("_bid")
+            res.append(r)
+        return res
+
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def run_model(self, frames_dev, center3d_override=None):
@@ -223,19 +348,23 @@ class BEV(torch.nn.Module):
            "regress")
 
     @torch.no_grad()
-    def run_post(self, B, offsets, img_max_side=512.0):
+    def run_post(self, B, offsets, img_max_side=512.0, b=None, o=None, cap=None, count=None):
         """SMPLA_parser + projection + the two per-frame filters (bev/main.py:172-180), then row compaction.  ``offsets``:
         one pad info for every frame (suppression with ``img_max_side``), or a device [B,6] table with one row per frame
-        (each frame projects and suppresses with its own size)."""
-        lib, b, o, sp = self.lib, self.buf, self.out, C.c_void_p(self.stream.cuda_stream)
-        cap = B * MAX_PERSON
+        (each frame projects and suppresses with its own size).  b / o / cap / count: the row buffers (default: the
+        regressor's rows)."""
+        lib, sp = self.lib, C.c_void_p(self.stream.cuda_stream)
+        b = self.buf if b is None else b
+        o = self.out if o is None else o
+        cap = B * MAX_PERSON if cap is None else cap
+        count = b["count"] if count is None else count
         if not self.calc_smpl:
             return
         st = self.stream.cuda_stream
-        self.smpla.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts"], b["joints"], st)
-        self.smil.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts_smil"], b["joints_smil"], st)
+        self.smpla.forward(b["betas"], b["thetas"], cap, count, True, b["smpl_ws"], b["verts"], b["joints"], st)
+        self.smil.forward(b["betas"], b["thetas"], cap, count, True, b["smpl_ws"], b["verts_smil"], b["joints_smil"], st)
         args = (_ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]), _ptr(b["joints"]), _ptr(b["cam"]),
-                _ptr(b["cam_trans"]), _ptr(b["batch_ids"]), B, cap, _ptr(b["count"]))
+                _ptr(b["cam_trans"]), _ptr(b["batch_ids"]), B, cap, _ptr(count))
         if isinstance(offsets, torch.Tensor) and offsets.dim() == 2:
             _lib.check(lib.b200romp_bev_post_frames(*args, _ptr(offsets), float(self.settings.nms_thresh),
                                                     float(self.settings.relative_scale_thresh), _ptr(b["pj2d_org"]), _ptr(b["keep"]),
@@ -277,10 +406,11 @@ class BEV(torch.nn.Module):
         return self._result(src, n, src["batch_ids"][:n], to_numpy)
 
     @torch.no_grad()
-    def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0):
+    def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0, signal_IDs=None):
         """frames [B,512,512,3] padded+resized like img_preprocess.  ``offsets``: one pad info [top,bottom,left,right,h,w]
         for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
-        suppressing with its own max(h, w) (``img_max_side`` is not used)."""
+        suppressing with its own max(h, w) (``img_max_side`` is not used).  With -t the frames are consecutive video
+        frames, tracked and smoothed in order (``signal_IDs``: one per frame, default 0); the result adds ``track_ids``."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         B = frames.shape[0]
@@ -290,18 +420,28 @@ class BEV(torch.nn.Module):
             fd.copy_(frames, non_blocking=True)
             offsets = frame_offsets(offsets, self.pad_table, B)
             self.run_model(fd, center3d_override)
-            self.run_post(B, offsets, img_max_side)
+            if self.temporal:
+                self.run_temporal(B, [0] * B if signal_IDs is None else list(signal_IDs))
+                self.run_post_temporal(B, offsets, img_max_side)
+            else:
+                self.run_post(B, offsets, img_max_side)
+        if self.temporal:
+            out, rows = self._collect_temporal(B, to_numpy)
+            out.pop("_bid")
+            return out if rows else None
         return self.collect(to_numpy)
 
     @torch.no_grad()
-    def forward_images(self, images, to_numpy=True, center3d_override=None):
+    def forward_images(self, images, to_numpy=True, center3d_override=None, signal_IDs=None):
         """Batched ``forward`` on raw images of any sizes (HxWx3 uint8 BGR: numpy arrays, host or device tensors): a list
         of the same length, element i the result for images[i] (dict or None; nothing is printed for normal images).
         Normal images run in chunks of at most ``max_batch`` through one preprocessing kernel per chunk (the GPU kernel,
         not the host OpenCV resize of ``forward``) and b200romp_bev_post_frames, each frame with its own pad info and
         suppression threshold; element i then equals ``forward_batch`` on image i's GPU-preprocessed frame with its pad
         info and ``img_max_side = max(h, w)``.  In crowd mode images with w/h >= 2 go one by one through
-        ``process_long_image``.  center3d_override: optional device [n_normal,64,128,128] for the normal images in order."""
+        ``process_long_image``.  center3d_override: optional device [n_normal,64,128,128] for the normal images in order.
+        With -t the normal images are consecutive video frames (``signal_IDs``: one per image, default 0), tracked and
+        smoothed in list order; wide crowd-mode images are neither tracked nor smoothed (bev/main.py:140-143)."""
         imgs = [image_tensor(x) for x in images]
         res = [None] * len(imgs)
         normal = []
@@ -317,12 +457,13 @@ class BEV(torch.nn.Module):
             after_producers(self.stream, self.tdevice, center3d_override)
         for c0 in range(0, len(normal), self.max_batch):
             idx = normal[c0:c0 + self.max_batch]
+            sigs = [0 if signal_IDs is None else signal_IDs[i] for i in idx]
             for i, r in zip(idx, self._forward_chunk([imgs[i] for i in idx], to_numpy,
-                                                     None if center3d_override is None else center3d_override[c0:c0 + len(idx)])):
+                                                     None if center3d_override is None else center3d_override[c0:c0 + len(idx)], sigs)):
                 res[i] = r
         return res
 
-    def _forward_chunk(self, imgs, to_numpy, center3d_override):
+    def _forward_chunk(self, imgs, to_numpy, center3d_override, signal_IDs=None):
         """One chunk of normal images: staging + one H2D, batched preprocessing, model, per-frame post; one host sync."""
         B = len(imgs)
         # the previous chunk ended in a host sync: the pinned buffer is free, and self.stream is the last reader of both
@@ -334,7 +475,14 @@ class BEV(torch.nn.Module):
                 self.raw.upload(total)
             preprocess_bgr_batch(self.lib, imgs, offs, self.raw.dev, fd, self.pad_table, self.stream.cuda_stream)
             self.run_model(fd, center3d_override)
-            self.run_post(B, self.pad_table[:B])
+            if self.temporal:
+                self.run_temporal(B, signal_IDs)
+                self.run_post_temporal(B, self.pad_table[:B])
+            else:
+                self.run_post(B, self.pad_table[:B])
+        if self.temporal:
+            out, rows = self._collect_temporal(B, to_numpy)
+            return self._split_temporal(out, B, rows, to_numpy)
         out = self.collect(to_numpy)
         if out is None:
             return [None] * B
@@ -459,7 +607,7 @@ class BEV(torch.nn.Module):
                 raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
             return self.process_long_image(image)
         inp, pad = img_preprocess(image)
-        out = self.forward_batch(torch.from_numpy(inp), offsets=pad, img_max_side=float(max(image.shape[:2])))
+        out = self.forward_batch(torch.from_numpy(inp), offsets=pad, img_max_side=float(max(image.shape[:2])), signal_IDs=[signal_ID])
         if out is None:
             print("No person detected!")                                       # bev/model.py:239
             return None
@@ -469,5 +617,7 @@ class BEV(torch.nn.Module):
         try:
             if getattr(self, "h", None):
                 self.lib.b200romp_bev_destroy(self.h)
+            if getattr(self, "trk", None):
+                self.lib.b200romp_bev_tracker_destroy(self.trk)
         except Exception:
             pass

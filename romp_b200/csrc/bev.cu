@@ -20,13 +20,13 @@
 
 #include "common.cuh"
 #include "rot6d.cuh"
+#include "bev_cam.cuh"
 
 namespace b200romp {
 
 constexpr int kD = 64, kS = 128, kVol = kD * kS * kS;
 constexpr int kCandCap = 4096;          // local maxima above threshold kept per frame before the top-64 sort
 constexpr int kMaxP = 64;
-constexpr float kTanFov = 0.57735026919f;   // tan(radians(60/2)), bev/post_parser.py:109
 
 struct BevDev {
   const float* center_ref;   // [56]  w1[27] b1 w2[27] b2   (BatchNorm3d folded)
@@ -394,27 +394,28 @@ __global__ void __launch_bounds__(128) bev_project_kernel(const float* __restric
   pj2d_org[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f - top;
 }
 
-// [start, start + n) = the rows of frame b (rows are grouped by frame, in frame order); n capped at 64
-__device__ __forceinline__ void frame_rows(const long long* __restrict__ batch_ids, int N, int b, int* s_start, int* s_n) {
+// [start, start + n) = the rows of frame b (rows are grouped by frame, in frame order); n capped at cap
+__device__ __forceinline__ void frame_rows(const long long* __restrict__ batch_ids, int N, int b, int* s_start, int* s_n, int cap = kMaxP) {
   int s = 0;
   while (s < N && batch_ids[s] < b) ++s;
   int e = s;
   while (e < N && batch_ids[e] == b) ++e;
-  *s_start = s; *s_n = min(e - s, kMaxP);
+  *s_start = s; *s_n = min(e - s, cap);
 }
 
-// Both reference post-filters on one frame's (<= 64) persons [st, st + nf), by the whole CTA (256 threads).  Persons with
+// Both reference post-filters on one frame's (<= CAP) persons [st, st + nf), by the whole CTA (256 threads).  Persons with
 // s_drop[i] set on entry take part in neither filter (the long-image boundary drop).  On return s_removed[i] = 1 for every
 // person that is dropped or filtered out.
 //   suppressing_redundant_prediction_via_projection (bev/post_parser.py:167-198): every pair below the threshold at once;
 //     conf == nullptr removes the smaller scale (cam[:,0]) of the pair, else the lower center_confs (conf_based=True, :191-193);
 //     on a tie the later person
 //   remove_outlier(relative_scale_thresh, scale_thresh) (:200-222)
+template <int CAP = kMaxP>
 __device__ void postfilter_frame(const float* __restrict__ pj2d_org, const float* __restrict__ cam, const float* __restrict__ cam_trans,
                                  const float* __restrict__ conf, int st, int nf, float nms_thr_px, float rel_scale_thresh,
                                  float scale_thresh, const int* s_drop, int* s_removed, int* s_kept, float* s_mean, int* s_nk) {
   const int tid = threadIdx.x;
-  if (tid < kMaxP) s_removed[tid] = tid < nf ? s_drop[tid] : 0;
+  if (tid < CAP) s_removed[tid] = tid < nf ? s_drop[tid] : 0;
   __syncthreads();
   if (nf > 1) {
     for (int pr = tid; pr < nf * nf; pr += blockDim.x) {
@@ -466,25 +467,27 @@ __device__ void postfilter_frame(const float* __restrict__ pj2d_org, const float
   }
 }
 
-// one CTA per frame: both reference post-filters on that frame's (<= 64) persons, then flags for the survivors
+// one CTA per frame: both reference post-filters on that frame's (<= CAP) persons, then flags for the survivors.  CAP is
+// 64 for the regressor's rows and 128 for the rows of BEV's video mode (two rows per detection at most)
+template <int CAP>
 __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
                                                              const float* __restrict__ cam_trans, const long long* __restrict__ batch_ids,
                                                              const int* __restrict__ d_count, float nms_thr_px, float rel_scale_thresh,
                                                              const float* __restrict__ pad_tab, float nms_thresh, int* __restrict__ keep) {
   __shared__ int s_start, s_n;
-  __shared__ int s_drop[kMaxP], s_removed[kMaxP], s_kept[kMaxP], s_nk;
-  __shared__ float s_mean[kMaxP];
+  __shared__ int s_drop[CAP], s_removed[CAP], s_kept[CAP], s_nk;
+  __shared__ float s_mean[CAP];
   const int b = blockIdx.x, tid = threadIdx.x;
   if (pad_tab) {                       // this frame's own threshold nms_thresh * max(h, w) / 640 (bev/post_parser.py:186-187)
     const float h = pad_tab[b * 6 + 4], w = pad_tab[b * 6 + 5];
     nms_thr_px = __fdiv_rn(__fmul_rn(nms_thresh, h > w ? h : w), 640.f);
   }
-  if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n);
-  if (tid < kMaxP) s_drop[tid] = 0;
+  if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n, CAP);
+  if (tid < CAP) s_drop[tid] = 0;
   __syncthreads();
   const int st = s_start, nf = s_n;
   if (nf == 0) return;
-  postfilter_frame(pj2d_org, cam, cam_trans, nullptr, st, nf, nms_thr_px, rel_scale_thresh, 0.25f, s_drop, s_removed, s_kept, s_mean, &s_nk);
+  postfilter_frame<CAP>(pj2d_org, cam, cam_trans, nullptr, st, nf, nms_thr_px, rel_scale_thresh, 0.25f, s_drop, s_removed, s_kept, s_mean, &s_nk);
   if (tid < nf) keep[st + tid] = s_removed[tid] ? 0 : 1;
 }
 
@@ -605,9 +608,9 @@ __global__ void __launch_bounds__(128) bev_long_project_kernel(const float* __re
                                                                int* __restrict__ removed) {
   const int n = blockIdx.x, j = threadIdx.x;
   if (n >= *d_count) return;
-  // denormalize_cam_params_to_trans (bev/post_parser.py:114-128), rounded op by op like the torch ops
-  const float depth = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(cam[n * 3], kTanFov), 1e-3f));
-  const float tx = __fmul_rn(__fmul_rn(cam[n * 3 + 2], depth), kTanFov), ty = __fmul_rn(__fmul_rn(cam[n * 3 + 1], depth), kTanFov);
+  float tr[3];
+  bev_cam_trans_rn(cam + n * 3, tr);                    // denormalize_cam_params_to_trans (bev/post_parser.py:114-128)
+  const float tx = tr[0], ty = tr[1], depth = tr[2];
   if (j == 0) {
     cam_trans[n * 3 + 0] = tx; cam_trans[n * 3 + 1] = ty; cam_trans[n * 3 + 2] = depth;
     removed[n] = 0;
@@ -878,8 +881,13 @@ static int bev_post(const float* betas, const float* verts_smil, const float* jo
   }
   bev_project_kernel<<<capacity, 128, 0, stream>>>(joints, cam_trans, d_count, size, left, top, pad_table, batch_ids, pj2d_org);
   B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
-  bev_postfilter_kernel<<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
-                                                   rel_scale_thresh, pad_table, nms_thresh, keep);
+  if (capacity > batch * kMaxP)
+    bev_postfilter_kernel<2 * kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count,
+                                                                nms_thresh * img_max_side / 640.f, rel_scale_thresh, pad_table,
+                                                                nms_thresh, keep);
+  else
+    bev_postfilter_kernel<kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
+                                                            rel_scale_thresh, pad_table, nms_thresh, keep);
   bev_compact_kernel<<<1, 32, 0, stream>>>(keep, d_count, sel, d_count_out);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;

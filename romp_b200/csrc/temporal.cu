@@ -10,11 +10,9 @@
 // host logic in romp_b200/temporal.py; this file only needs the slot index of every person.
 #include "common.cuh"
 #include "rot6d.cuh"
+#include "one_euro.cuh"
 
 namespace b200romp {
-
-constexpr int kOeCh = 9 + 69 + 16 + 3;       // global-rot matrix | body pose | betas (up to 16) | cam
-constexpr int kOeGlob = 0, kOePose = 9, kOeBeta = 78, kOeCam = 94;
 
 struct OeState {
   float* prev_raw;      // [slots][kOeCh]  LowPassFilter.prev_raw_value of the x filter
@@ -22,12 +20,6 @@ struct OeState {
   float* prev_dx;       // [slots][kOeCh]  prev_filtered_value of the dx filter
   int* seen;            // [slots] 0 = the next sample initialises the filters
 };
-
-__device__ __forceinline__ float oe_alpha(float cutoff, float freq) {     // OneEuroFilter.compute_alpha, utils.py:227-230
-  const float te = 1.0f / freq;
-  const float tau = 1.0f / (2.0f * 3.14159265358979323846f * cutoff);
-  return 1.0f / (1.0f + tau / te);
-}
 
 // block = one person, thread = one filtered scalar
 __global__ void __launch_bounds__(128) one_euro_kernel(OeState st, const int* __restrict__ slot, int n_host, const int* __restrict__ d_count,
@@ -40,21 +32,7 @@ __global__ void __launch_bounds__(128) one_euro_kernel(OeState st, const int* __
   if (sl < 0) return;
   __shared__ float s_R[9];
   const int t = threadIdx.x;
-  if (t < 9) {
-    // utils.batch_rodrigues (:493-505) + quat2mat (:507-533) of the global rotation
-    const float* a = thetas + (size_t)i * 72;
-    const float ex = a[0] + 1e-8f, ey = a[1] + 1e-8f, ez = a[2] + 1e-8f;
-    const float nrm = sqrtf(ex * ex + ey * ey + ez * ez);
-    const float ux = a[0] / nrm, uy = a[1] / nrm, uz = a[2] / nrm;
-    const float h = nrm * 0.5f, c = cosf(h), s = sinf(h);
-    float w = c, x = s * ux, y = s * uy, z = s * uz;
-    const float qn = sqrtf(w * w + x * x + y * y + z * z);
-    w /= qn; x /= qn; y /= qn; z /= qn;
-    const float w2 = w * w, x2 = x * x, y2 = y * y, z2 = z * z, wx = w * x, wy = w * y, wz = w * z, xy = x * y, xz = x * z, yz = y * z;
-    const float R[9] = {w2 + x2 - y2 - z2, 2 * xy - 2 * wz, 2 * wy + 2 * xz, 2 * wz + 2 * xy, w2 - x2 + y2 - z2, 2 * yz - 2 * wx,
-                        2 * xz - 2 * wy, 2 * wx + 2 * yz, w2 - x2 - y2 + z2};
-    s_R[t] = R[t];
-  }
+  if (t == 0) oe_rodrigues(thetas + (size_t)i * 72, s_R);      // utils.batch_rodrigues (:493-505) + quat2mat (:507-533)
   __syncthreads();
   float x = 0.f, mincut = smooth_coeff;
   bool active = true;
@@ -66,19 +44,7 @@ __global__ void __launch_bounds__(128) one_euro_kernel(OeState st, const int* __
   float y = x;
   if (active) {
     const size_t o = (size_t)sl * kOeCh + t;
-    if (st.seen[sl]) {
-      const float dx = (x - st.prev_raw[o]) * freq;                                   // :233-234
-      const float ad = oe_alpha(1.0f, freq);
-      const float edx = ad * dx + (1.0f - ad) * st.prev_dx[o];                         // dx_filter.process, :209-214
-      const float cutoff = mincut + 0.7f * fabsf(edx);                                 // :237-242
-      const float ax = oe_alpha(cutoff, freq);
-      y = ax * x + (1.0f - ax) * st.prev_x[o];                                         // x_filter.process
-      st.prev_dx[o] = edx;
-    } else {
-      st.prev_dx[o] = 0.0f;                                                            // first sample: dx = 0.0, s = value
-    }
-    st.prev_raw[o] = x;
-    st.prev_x[o] = y;
+    y = oe_step(x, mincut, freq, st.seen[sl] != 0, &st.prev_raw[o], &st.prev_x[o], &st.prev_dx[o]);
   }
   if (t < kOePose) s_R[t] = y;
   else if (t < kOeBeta) thetas[(size_t)i * 72 + 3 + (t - kOePose)] = y;
