@@ -15,7 +15,8 @@ struct S2Maps {
 
 struct TcConvPlan {
   int kind = 0;                 // kernel family: 10 = 1x1, 30 = 3x3, 32 = 3x3 stride 2, 33 = u8 stem, 13 = conv1d,
-                                // 60 = fused 3x3 BasicBlock (conv_block_tc.cu); 0 = none
+                                // 60 = fused 3x3 BasicBlock (conv_block_tc.cu), 70 = fused Bottleneck
+                                // (conv_bottleneck_tc.cu); 0 = none
   int cin = 0, cout = 0, nt = 0;  // channels, output channels per CTA
   int eb = 2;                   // operand element bytes: 2 = bf16, 4 = fp32 storage consumed as TF32
   int grid_x = 0, grid_y = 0, stages = 0;
@@ -28,8 +29,10 @@ struct TcConvPlan {
   unsigned kmask = 0xFFFFFFFFu;
   const void* encoded_in = nullptr;   // conv1d engine: input pointer / batch the tensor map was encoded for
   int encoded_batch = 0;
-  void* d_wpack2 = nullptr;           // fused block: conv2's weight image (d_wpack holds conv1's)
-  const float* d_bias1 = nullptr;     // fused block: conv1's bias [64] (conv2's is ConvParams::bias)
+  void* d_wpack2 = nullptr;           // fused block / Bottleneck: conv2's weight image (d_wpack holds conv1's)
+  void* d_wpack3 = nullptr;           // fused Bottleneck: conv3's weight image
+  const float* d_bias1 = nullptr;     // fused block / Bottleneck: conv1's bias [64] (the last conv's is ConvParams::bias)
+  const float* d_bias2 = nullptr;     // fused Bottleneck: conv2's bias [64]
   int fold = 0;                       // set before prepare: runs on the pixel-pair view (net.cu fold_pixel_pairs)
   std::string describe() const;
 };
@@ -55,5 +58,19 @@ bool tc_block_supported(const ConvParams& p);
 int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
                      TcConvPlan* plan, std::vector<void*>* allocs);
 int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);
+// fused Bottleneck engine (conv_bottleneck_tc.cu): y = relu(W3 relu(W2 * relu(W1 x + b1) + b2) + b3 + x) with 1x1 256 -> 64,
+// 3x3 stride-1 64 -> 64 and 1x1 64 -> 256 convs, bf16 NHWC.  `p` describes the block as one op: input and residual x (the
+// same 256-channel slice), output y, bias b3.
+// `BottleneckMids` are set when other ops of the net also read t1 or t2 (whole 64-channel slices of bf16 NHWC tensors at
+// the block's resolution); the kernel then writes them as well.
+struct BottleneckMids {
+  __nv_bfloat16* t1 = nullptr;
+  __nv_bfloat16* t2 = nullptr;
+  int t1_C = 0, t2_C = 0;
+};
+bool tc_bottleneck_supported(const ConvParams& p);
+int tc_bottleneck_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, const float* b2,
+                          const float* w3_oihw, int sm_count, TcConvPlan* plan, std::vector<void*>* allocs);
+int tc_bottleneck_launch(const TcConvPlan& plan, const ConvParams& p, const BottleneckMids& mids, cudaStream_t stream);
 
 }  // namespace b200romp

@@ -37,10 +37,11 @@ struct Tensor {
   size_t frame_bytes() const { return (size_t)H * W * C * dtype_size(dtype); }
 };
 
-// The kernel that runs an op.  Sum and MaxPool are set when the op is added, WgmmaBlock by fuse_basic_blocks; every other
+// The kernel that runs an op.  Sum and MaxPool are set when the op is added, WgmmaBlock by fuse_basic_blocks,
+// WgmmaBottleneck by fuse_bottlenecks; every other
 // conv is Simt until choose_kernel decides at finalize.  Generic7x7 and Deconv4x4 are the CUDA-core kernels of
 // resnet_ops.cu; a Wgmma or WgmmaBlock plan with tc.fold runs on the pixel-pair view (fold_pixel_pairs).
-enum class Kernel { Sum, MaxPool, Simt, Generic7x7, Deconv4x4, Wgmma, WgmmaStem, WgmmaConv1d, WgmmaBlock };
+enum class Kernel { Sum, MaxPool, Simt, Generic7x7, Deconv4x4, Wgmma, WgmmaStem, WgmmaConv1d, WgmmaBlock, WgmmaBottleneck };
 
 struct Op {
   Kernel kernel = Kernel::Simt;
@@ -56,9 +57,24 @@ struct Op {
   // conv2's, `mid` is the intermediate tensor that no longer gets a buffer
   int mid = -1;
   std::vector<float> w2_host, b2_host;
+  // WgmmaBottleneck: as WgmmaBlock for its first two convs (d.cout = 256, bias = b3), w3_host / b3_host conv3's, `mid2`
+  // conv2's output.  An intermediate that other ops read as well is stored (store_mid, store_mid2) and gets a buffer.
+  int mid2 = -1;
+  bool store_mid = false, store_mid2 = false;
+  std::vector<float> w3_host, b3_host;
 };
 
-static bool on_wgmma(Kernel k) { return k == Kernel::Wgmma || k == Kernel::WgmmaStem || k == Kernel::WgmmaConv1d || k == Kernel::WgmmaBlock; }
+// the tensors an op writes: its output, and a fused Bottleneck's stored intermediates
+static std::vector<int> op_outputs(const Op& op) {
+  std::vector<int> o{op.d.out};
+  if (op.store_mid) o.push_back(op.mid);
+  if (op.store_mid2) o.push_back(op.mid2);
+  return o;
+}
+
+static bool on_wgmma(Kernel k) {
+  return k == Kernel::Wgmma || k == Kernel::WgmmaStem || k == Kernel::WgmmaConv1d || k == Kernel::WgmmaBlock || k == Kernel::WgmmaBottleneck;
+}
 
 }  // namespace b200romp
 
@@ -324,6 +340,18 @@ static int enqueue_op(b200romp_net* net, Op& op, int batch, cudaStream_t stream)
     case Kernel::WgmmaStem: return tc_stem_launch(op.tc, p, stream);
     case Kernel::WgmmaConv1d: return tc_conv1d_launch(op.tc, p, stream);
     case Kernel::WgmmaBlock: return tc_block_launch(op.tc, p, stream);
+    case Kernel::WgmmaBottleneck: {
+      BottleneckMids mids;
+      if (op.store_mid) {
+        mids.t1 = static_cast<__nv_bfloat16*>(net->tensors[op.mid].ptr);
+        mids.t1_C = net->tensors[op.mid].C;
+      }
+      if (op.store_mid2) {
+        mids.t2 = static_cast<__nv_bfloat16*>(net->tensors[op.mid2].ptr);
+        mids.t2_C = net->tensors[op.mid2].C;
+      }
+      return tc_bottleneck_launch(op.tc, p, mids, stream);
+    }
   }
   return B200ROMP_EINVAL;
 }
@@ -392,25 +420,45 @@ static unsigned fold_kmask() {
 // Ops i, i+1 fuse when conv2 reads exactly conv1's output, that tensor is internal and read by nothing else, conv2's
 // residual is conv1's input slice, and the block kernel supports the fused op.  A caller that binds the intermediate as an
 // external tensor keeps the two convs.
-static bool is_bf16_block_conv(const b200romp_net* net, const Op& op) {
+// a bf16 NHWC stride-1 ReLU conv of kernel size `ksize` from cin to cout channels that a fused wgmma kernel may take
+static bool is_bf16_relu_conv(const b200romp_net* net, const Op& op, int ksize, int cin, int cout) {
   const b200romp_conv_desc& d = op.d;
   const Tensor& ti = net->tensors[d.in];
   const Tensor& to = net->tensors[d.out];
-  return d.ksize == 3 && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
+  return d.ksize == ksize && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
          (d.engine == B200ROMP_ENGINE_AUTO || d.engine == B200ROMP_ENGINE_WGMMA) && ti.dtype == B200ROMP_BF16 &&
-         to.dtype == B200ROMP_BF16 && !to.nchw && d.cin == d.cout && (d.cin == 64 || d.cin == 32);
+         to.dtype == B200ROMP_BF16 && !to.nchw && d.cin == cin && d.cout == cout;
+}
+
+static bool is_bf16_block_conv(const b200romp_net* net, const Op& op) {
+  return is_bf16_relu_conv(net, op, 3, 64, 64) || is_bf16_relu_conv(net, op, 3, 32, 32);
+}
+
+// how many ops read / write each tensor
+static void count_accesses(const b200romp_net* net, std::vector<int>* reads, std::vector<int>* writes) {
+  reads->assign(net->tensors.size(), 0);
+  writes->assign(net->tensors.size(), 0);
+  for (const Op& op : net->ops) {
+    ++(*reads)[op.d.in];
+    ++(*writes)[op.d.out];
+    if (op.kernel == Kernel::Sum)
+      for (int k = 0; k < op.sum.n_terms; ++k) ++(*reads)[op.sum.term[k]];
+    else if (op.d.res >= 0) ++(*reads)[op.d.res];
+  }
+}
+
+// `t`, the output of op a and the whole input of op b, can be produced and consumed inside a fused kernel: internal,
+// whole-tensor, written by a only and not b's residual.  Ops after b may read it too.
+static bool fusable_intermediate(const b200romp_net* net, const Op& a, const Op& b, const std::vector<int>& writes) {
+  const int t = a.d.out;
+  const Tensor& tt = net->tensors[t];
+  return b.d.in == t && b.d.in_c_off == 0 && a.d.out_c_off == 0 && tt.C == a.d.cout && !tt.external && !tt.constant &&
+         writes[t] == 1 && b.d.res != t;
 }
 
 static void fuse_basic_blocks(b200romp_net* net) {
-  const int nT = (int)net->tensors.size();
-  std::vector<int> reads(nT, 0), writes(nT, 0);
-  for (const Op& op : net->ops) {
-    ++reads[op.d.in];
-    ++writes[op.d.out];
-    if (op.kernel == Kernel::Sum)
-      for (int k = 0; k < op.sum.n_terms; ++k) ++reads[op.sum.term[k]];
-    else if (op.d.res >= 0) ++reads[op.d.res];
-  }
+  std::vector<int> reads, writes;
+  count_accesses(net, &reads, &writes);
   std::vector<Op> fused;
   fused.reserve(net->ops.size());
   for (size_t i = 0; i < net->ops.size(); ++i) {
@@ -445,6 +493,62 @@ static void fuse_basic_blocks(b200romp_net* net) {
           f.b2_host = std::move(b.b_host);
           fused.push_back(std::move(f));
           ++i;
+          continue;
+        }
+      }
+    }
+    fused.push_back(std::move(a));
+  }
+  net->ops = std::move(fused);
+}
+
+// ResNet Bottlenecks relu(conv3(relu(conv2(relu(conv1(x))))) + x) with identity residual, 1x1 256->64, 3x3 stride-1 64->64 and
+// 1x1 64->256 bf16 convs (HRNet layer1.1 .. layer1.3), become one op on the fused Bottleneck kernel (conv_bottleneck_tc.cu):
+// the two 64-channel intermediates never reach HBM and x is read once.  Ops i, i+1, i+2 fuse when each intermediate is
+// internal and written only by its conv, conv3's residual is conv1's input slice, the three run on one lane, and the
+// Bottleneck kernel supports the fused op.  An intermediate that later ops read as well is also written by the kernel.
+static void fuse_bottlenecks(b200romp_net* net) {
+  std::vector<int> reads, writes;
+  count_accesses(net, &reads, &writes);
+  std::vector<Op> fused;
+  fused.reserve(net->ops.size());
+  for (size_t i = 0; i < net->ops.size(); ++i) {
+    Op& a = net->ops[i];
+    if (i + 2 < net->ops.size()) {
+      Op& b = net->ops[i + 1];
+      Op& c = net->ops[i + 2];
+      const int x = a.d.in;
+      const bool ok = a.kernel == Kernel::Simt && b.kernel == Kernel::Simt && c.kernel == Kernel::Simt &&
+                      is_bf16_relu_conv(net, a, 1, 256, 64) && is_bf16_relu_conv(net, b, 3, 64, 64) &&
+                      is_bf16_relu_conv(net, c, 1, 64, 256) && a.d.res < 0 && b.d.res < 0 && a.lane == b.lane &&
+                      b.lane == c.lane && fusable_intermediate(net, a, b, writes) && fusable_intermediate(net, b, c, writes) &&
+                      c.d.res == x && c.d.res_c_off == a.d.in_c_off &&
+                      !c.d.res_broadcast && !net->tensors[x].external && !net->tensors[c.d.out].external;
+      if (ok) {
+        Op f;
+        f.kernel = Kernel::WgmmaBottleneck;
+        f.d = a.d;
+        f.d.cout = c.d.cout;
+        f.d.out = c.d.out;
+        f.d.out_c_off = c.d.out_c_off;
+        f.d.res = x;
+        f.d.res_c_off = c.d.res_c_off;
+        ConvParams p;
+        fill_params(net, f, 1, true, &p);
+        if (tc_bottleneck_supported(p)) {
+          f.mid = a.d.out;
+          f.mid2 = b.d.out;
+          f.store_mid = reads[f.mid] > 1;
+          f.store_mid2 = reads[f.mid2] > 1;
+          f.lane = a.lane;
+          f.w_host = std::move(a.w_host);
+          f.b_host = std::move(a.b_host);
+          f.w2_host = std::move(b.w_host);
+          f.b2_host = std::move(b.b_host);
+          f.w3_host = std::move(c.w_host);
+          f.b3_host = std::move(c.b_host);
+          fused.push_back(std::move(f));
+          i += 2;
           continue;
         }
       }
@@ -499,7 +603,9 @@ static int prepare_op(b200romp_net* net, Op& op) {
     fold_pixel_pairs(&w, &b);
     if (op.kernel == Kernel::WgmmaBlock) fold_pixel_pairs(&w2, &b2);
   }
-  std::vector<float> bias = op.kernel == Kernel::WgmmaBlock ? b2 : b;   // a block's bias is conv2's
+  std::vector<float> b3 = std::move(op.b3_host);
+  // a block's bias is conv2's, a Bottleneck's conv3's
+  std::vector<float> bias = op.kernel == Kernel::WgmmaBlock ? b2 : op.kernel == Kernel::WgmmaBottleneck ? b3 : b;
   op.coutPad = ((int)bias.size() + 63) / 64 * 64;
   bias.resize(op.coutPad, 0.f);
   int rc = upload(net, bias, &op.d_bias);
@@ -525,6 +631,10 @@ static int prepare_op(b200romp_net* net, Op& op) {
     case Kernel::WgmmaStem: return tc_stem_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
     case Kernel::WgmmaConv1d: return tc_conv1d_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
     case Kernel::WgmmaBlock: return tc_block_prepare(p, w.data(), b.data(), w2.data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaBottleneck: {
+      const std::vector<float> w3 = std::move(op.w3_host);
+      return tc_bottleneck_prepare(p, w.data(), b.data(), w2.data(), b2.data(), w3.data(), net->sm_count, &op.tc, &net->device_allocs);
+    }
     default: return B200ROMP_OK;
   }
 }
@@ -533,13 +643,16 @@ int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   B2R_REQUIRE(net && !net->finalized && max_batch > 0, "finalize: bad arguments");
   B2R_CUDA_OK(cudaSetDevice(net->device));
   fuse_basic_blocks(net);   // before liveness: a fused block's intermediate gets no buffer
+  fuse_bottlenecks(net);    // likewise a fused Bottleneck's two, unless other ops read them
   const int nT = (int)net->tensors.size(), nO = (int)net->ops.size();
   // ---- liveness over the linear op order
   for (int i = 0; i < nO; ++i) {
     const b200romp_conv_desc& d = net->ops[i].d;
-    Tensor& to = net->tensors[d.out];
-    if (to.first_def < 0) to.first_def = i;
-    to.last_use = std::max(to.last_use, i);
+    for (int t : op_outputs(net->ops[i])) {
+      Tensor& to = net->tensors[t];
+      if (to.first_def < 0) to.first_def = i;
+      to.last_use = std::max(to.last_use, i);
+    }
     net->tensors[d.in].last_use = std::max(net->tensors[d.in].last_use, i);
     if (d.res >= 0) net->tensors[d.res].last_use = std::max(net->tensors[d.res].last_use, i);
     if (net->ops[i].kernel == Kernel::Sum)
@@ -570,9 +683,9 @@ int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   }
   size_t total = 0;
   for (int i = 0; i < nO; ++i) {
-    const int t = net->ops[i].d.out;
-    const Tensor& tt = net->tensors[t];
-    if (!tt.external && !tt.constant && tt.first_def == i) {
+    for (int t : op_outputs(net->ops[i])) {
+      const Tensor& tt = net->tensors[t];
+      if (tt.external || tt.constant || tt.first_def != i) continue;
       const size_t bytes = (tt.frame_bytes() * max_batch + 1023) / 1024 * 1024;
       auto it = free_bufs.find(bytes);
       if (it != free_bufs.end()) {
@@ -642,15 +755,15 @@ static int enqueue_all_lanes(b200romp_net* net, int batch, cudaStream_t stream) 
       B2R_CUDA_OK(cudaStreamWaitEvent(st, net->fork_ev, 0));
       lane_used[lane] = true;
     }
-    std::vector<const void*> reads;
-    const void* write = net->tensors[op.d.out].ptr;
+    std::vector<const void*> reads, writes;
+    for (int t : op_outputs(op)) writes.push_back(net->tensors[t].ptr);
     auto add_read = [&](int t) { if (t >= 0 && !net->tensors[t].constant) reads.push_back(net->tensors[t].ptr); };
     add_read(op.d.in);
     if (op.kernel == Kernel::Sum) for (int k = 0; k < op.sum.n_terms; ++k) add_read(op.sum.term[k]);
     else add_read(op.d.res);
     std::vector<int> deps;
     for (const void* r : reads) { auto it = acc.find(r); if (it != acc.end() && it->second.writer >= 0) deps.push_back(it->second.writer); }
-    { auto it = acc.find(write); if (it != acc.end()) { if (it->second.writer >= 0) deps.push_back(it->second.writer); for (int r : it->second.readers) deps.push_back(r); } }
+    for (const void* w : writes) { auto it = acc.find(w); if (it != acc.end()) { if (it->second.writer >= 0) deps.push_back(it->second.writer); for (int r : it->second.readers) deps.push_back(r); } }
     std::sort(deps.begin(), deps.end());
     deps.erase(std::unique(deps.begin(), deps.end()), deps.end());
     bool cross = false;
@@ -664,9 +777,11 @@ static int enqueue_all_lanes(b200romp_net* net, int batch, cudaStream_t stream) 
     if (rc) break;
     B2R_CUDA_OK(cudaEventRecord(net->op_done[i], st));
     for (const void* r : reads) acc[r].readers.push_back((int)i);
-    Access& w = acc[write];
-    w.writer = (int)i;
-    w.readers.clear();
+    for (const void* wp : writes) {
+      Access& w = acc[wp];
+      w.writer = (int)i;
+      w.readers.clear();
+    }
   }
   // join: the user stream continues after the last op of every lane
   if (rc == B200ROMP_OK) {
@@ -794,6 +909,21 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
                  "bias1 bias2 [tc-block grid %d smem %d%s]\n",
                  i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
                  d.out_c_off, d.res, d.res_c_off, op.tc.grid_x, op.tc.smem_bytes, op.tc.fold ? " conv1 pixel-pairs conv2 pixel-pairs" : "");
+        break;
+      }
+      case Kernel::WgmmaBottleneck: {   // one launch, three convs: one line per conv, all with the op's number
+        const Tensor& tm = net->tensors[op.mid];
+        const Tensor& tm2 = net->tensors[op.mid2];
+        const char* fmt = "op%03zu wgmma   k%d s1 %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up1 relu1 "
+                          "[tc-bottleneck conv%d of k1-k3-k1 grid %d smem %d]\n";
+        snprintf(line, sizeof(line), fmt, i, 1, d.cin, tm.C, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, 0, -1, 1,
+                 op.tc.grid_x, op.tc.smem_bytes);
+        s += line;
+        snprintf(line, sizeof(line), fmt, i, 3, tm.C, tm2.C, op.mid, tm.H, tm.W, tm.C, 0, op.mid2, tm2.H, tm2.W, tm2.C, 0, -1, 2,
+                 op.tc.grid_x, op.tc.smem_bytes);
+        s += line;
+        snprintf(line, sizeof(line), fmt, i, 1, tm2.C, d.cout, op.mid2, tm2.H, tm2.W, tm2.C, 0, d.out, to.H, to.W, to.C, d.out_c_off,
+                 d.res, 3, op.tc.grid_x, op.tc.smem_bytes);
         break;
       }
       default:

@@ -8,7 +8,10 @@ the input channel slice, the output and the residual read once each, at the acti
 bf16, 4 otherwise; the few fp32 tensors of a bf16 net are counted at 2).  Low-intensity layers are bounded by these bytes,
 not by FLOPs, so GB/s is the rate to set against the HBM bandwidth.  A fused BasicBlock op (`block k3`, conv_block_tc.cu)
 counts the FLOPs of both convs and moves its input once and its output once: the intermediate stays in shared memory and
-the residual is the block's own input, read from the staged input tile, so neither adds bytes."""
+the residual is the block's own input, read from the staged input tile, so neither adds bytes.  A fused Bottleneck op
+(conv_bottleneck_tc.cu, one describe() line per conv under one op number, shown here as `bottleneck k1-k3-k1`) counts the algorithmic FLOPs of its three convs (not conv1's recompute on
+the tile halo) and moves its input once and its output once: both intermediates stay in shared memory and the residual,
+its own input, is read again from L2."""
 import argparse
 import os
 import re
@@ -42,7 +45,17 @@ def main():
         for k, t in ext.items():
             _lib.check(lib.b200romp_net_bind(nb.net, io[k], t.data_ptr()))
     us = nb.profile(B, args.iters)
-    lines = [l for l in nb.describe().splitlines() if l.startswith("op")]
+    lines = []
+    for l in nb.describe().splitlines():
+        if not l.startswith("op"):
+            continue
+        m = re.search(r"k\d s1 +(\d+)->(\d+) +in (t\d+\[\S+).*\[tc-bottleneck conv(\d)", l)
+        if m and m.group(4) != "1":   # conv2 / conv3 of the fused Bottleneck begun on the previous line: one op, one time
+            lines[-1] = lines[-1].replace("->?", f"->{m.group(2)}" + ("->?" if m.group(4) == "2" else ""))
+            continue
+        if m:
+            l = f"{l[:5]} wgmma   bottleneck k1-k3-k1 {m.group(1)}->{m.group(2)}->? in {m.group(3)}"
+        lines.append(l)
     rows = []
     for l, t in zip(lines, us):
         if " sum " in l:
@@ -52,6 +65,11 @@ def main():
         if mb:
             c0, c1, c2, H, W = (int(x) for x in mb.groups())
             rows.append((t, 2.0 * B * H * W * 9 * (c0 * c1 + c1 * c2), eb * B * H * W * (c0 + c2), l))
+            continue
+        mb = re.search(r"bottleneck k1-k3-k1 (\d+)->(\d+)->(\d+)->(\d+) in t\d+\[(\d+)x(\d+)x\d+\]", l)
+        if mb:
+            c0, c1, c2, c3, H, W = (int(x) for x in mb.groups())
+            rows.append((t, 2.0 * B * H * W * (c0 * c1 + 9 * c1 * c2 + c2 * c3), eb * B * H * W * (c0 + c3), l))
             continue
         m = re.search(r"k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x(\d+)x\d+\]", l)
         k, s, cin, cout, H, W = (int(x) for x in m.groups())
@@ -73,9 +91,9 @@ def main():
             a = cls.setdefault(f"sum @{ms.group(1)} c{ms.group(2)} terms{l.count('up')}", [0, 0.0, 0.0, 0.0])
             a[0] += 1; a[1] += t
             continue
-        mb = re.search(r"block k3 s1 (\d+->\d+->\d+) in t\d+\[(\d+)x", l)
+        mb = re.search(r"(block k3|bottleneck k1-k3-k1) (?:s1 )?(\d+->\d+->\d+(?:->\d+)?) in t\d+\[(\d+)x", l)
         if mb:
-            a = cls.setdefault(f"wgmma block k3 {mb.group(1)} @{mb.group(2)} res", [0, 0.0, 0.0, 0.0])
+            a = cls.setdefault(f"wgmma {mb.group(1)} {mb.group(2)} @{mb.group(3)} res", [0, 0.0, 0.0, 0.0])
             a[0] += 1; a[1] += t; a[2] += f; a[3] += nb_
             continue
         m = re.search(r"(wgmma|simt) +k(\d+) s(\d) +(\d+)->(\d+) +in t\d+\[(\d+)x", l)
