@@ -218,7 +218,8 @@ int b200romp_bev_bv_input(const float* maps_fv, const void* img_feats, int feats
 int b200romp_bev_center3d(b200romp_bev* bev, const float* maps_fv, const void* bv_out, int bv_dtype, int batch, float* tmp,
                           float* center3d, b200romp_stream stream);
 /* CenterMap3D.parse_3dcentermap (bev/post_parser.py:44-66): 5x5x5 NMS, top-64 per frame, > thresh.  Order: frame asc,
- * score desc (ties: voxel index asc).  Exact as long as a frame has <= 4096 local maxima above thresh. */
+ * score desc (ties: voxel index asc), exact and deterministic for any number of local maxima above thresh (a frame with
+ * more than 4096 of them takes a slower exact selection).  Stream-ordered, no host sync. */
 long long b200romp_bev_parse_workspace_bytes(int batch);
 int b200romp_bev_parse3d(const float* center3d, int batch, float thresh, int capacity, int* d_count, long long* batch_ids,
                          long long* czyx /*[cap,3]*/, float* conf, void* workspace, b200romp_stream stream);

@@ -161,16 +161,11 @@ __global__ void __launch_bounds__(256) bev_center3d_fused_kernel(const float* __
 }
 
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) bev_nms3d_kernel(const float* __restrict__ c3d, int B, float thresh,
-                                                        int* __restrict__ cand_count, int* __restrict__ cand_idx,
-                                                        float* __restrict__ cand_val) {
-  const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= (size_t)B * kVol) return;
-  const float v = c3d[idx];
-  if (!(v > thresh)) return;                       // det * (maxpool == det) > thresh  <=>  det > thresh and det is a maximum
-  const int vox = idx % kVol, b = idx / kVol;
+// det * (maxpool == det) > thresh  <=>  det > thresh and no voxel of its 5^3 window (inside the frame) is larger
+__device__ __forceinline__ bool nms3d_keep(const float* __restrict__ base, int vox, float thresh) {
+  const float v = base[vox];
+  if (!(v > thresh)) return false;
   const int x = vox % kS, y = (vox / kS) % kS, z = vox / (kS * kS);
-  const float* base = c3d + (size_t)b * kVol;
   for (int dz = -2; dz <= 2; ++dz) {
     const int zz = z + dz;
     if (zz < 0 || zz >= kD) continue;
@@ -180,31 +175,110 @@ __global__ void __launch_bounds__(256) bev_nms3d_kernel(const float* __restrict_
       for (int dx = -2; dx <= 2; ++dx) {
         const int xx = x + dx;
         if (xx < 0 || xx >= kS) continue;
-        if (base[((size_t)zz * kS + yy) * kS + xx] > v) return;
+        if (base[((size_t)zz * kS + yy) * kS + xx] > v) return false;
       }
     }
   }
+  return true;
+}
+
+// Appends every local maximum above thresh to its frame's candidate list (the first kCandCap of them, in arrival order)
+// and writes the frame's local-maximum bitmask (bit vox % 32 of word vox / 32), which select64 reads when a frame
+// has more than kCandCap maxima.  The grid covers B * kVol threads exactly, so every warp writes one whole mask word.
+__global__ void __launch_bounds__(256) bev_nms3d_kernel(const float* __restrict__ c3d, float thresh, int* __restrict__ cand_count,
+                                                        int* __restrict__ cand_idx, float* __restrict__ cand_val,
+                                                        uint32_t* __restrict__ max_mask) {
+  const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
+  const int vox = idx % kVol, b = idx / kVol;
+  const bool keep = nms3d_keep(c3d + (size_t)b * kVol, vox, thresh);
+  const uint32_t bits = __ballot_sync(0xffffffffu, keep);
+  if ((threadIdx.x & 31) == 0) max_mask[idx / 32] = bits;
+  if (!keep) return;
   const int slot = atomicAdd(&cand_count[b], 1);
   if (slot < kCandCap) {
     cand_idx[(size_t)b * kCandCap + slot] = vox;
-    cand_val[(size_t)b * kCandCap + slot] = v;
+    cand_val[(size_t)b * kCandCap + slot] = c3d[idx];
+  }
+}
+
+// Unique sort key of a local maximum: larger key = earlier in the parse order (value desc, voxel index asc).  The values
+// are > thresh >= 0, so their bit patterns order like the values.
+__device__ __forceinline__ unsigned long long parse_key(float v, int vox) {
+  return ((unsigned long long)__float_as_uint(v) << 32) | (0xFFFFFFFFu - (unsigned)vox);
+}
+
+// Exact top-64 of a frame with more than kCandCap local maxima (its candidate list then holds an arbitrary subset), by
+// the whole CTA (1024 threads) into s_key / s_idx [0, 64): an MSB-first radix select (8-bit digits) over the keys of all
+// the frame's maxima, read through the bitmask, finds the digits of the 64th-largest key until its digit bucket is taken
+// whole; the keys at or above that bucket are exactly the top 64.
+__device__ void select64(const float* __restrict__ vals, const uint32_t* __restrict__ mask, float* s_key, int* s_idx) {
+  __shared__ unsigned s_hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_rank, s_n, s_done;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  unsigned long long prefix = 0, pmask = 0;               // the digits of the 64th-largest key found so far
+  if (tid == 0) { s_rank = kMaxP; s_n = 0; }              // its rank among the keys that share those digits
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += blockDim.x) s_hist[i] = 0;
+    __syncthreads();
+    for (int w = warp; w < kVol / 32; w += nwarps) {      // one mask word (32 consecutive voxels) per warp step
+      const uint32_t bits = mask[w];
+      if (bits == 0) continue;
+      const int vox = w * 32 + lane;
+      const unsigned long long key = parse_key(vals[vox], vox);
+      const bool in = ((bits >> lane) & 1u) && (key & pmask) == prefix;
+      const unsigned digit = (unsigned)(key >> shift) & 255u;
+      const unsigned peers = __match_any_sync(0xffffffffu, in ? digit : 256u + lane);   // lanes with the same digit
+      if (in && lane == __ffs(peers) - 1) atomicAdd(&s_hist[digit], __popc(peers));
+    }
+    __syncthreads();
+    if (tid == 0) {                                       // the bucket that holds the rank-th largest key
+      int rank = s_rank, d = 255;
+      for (; d > 0 && (int)s_hist[d] < rank; --d) rank -= s_hist[d];
+      s_rank = rank;
+      s_done = (int)s_hist[d] == rank;
+      s_prefix = prefix | ((unsigned long long)d << shift);
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    pmask |= 255ull << shift;
+    if (s_done) break;
+  }
+  for (int w = warp; w < kVol / 32; w += nwarps) {        // 64 - rank keys above the bucket, rank keys in it
+    const uint32_t bits = mask[w];
+    if (bits == 0) continue;
+    const int vox = w * 32 + lane;
+    const float v = vals[vox];
+    if (((bits >> lane) & 1u) && (parse_key(v, vox) & pmask) >= prefix) {
+      const int slot = atomicAdd(&s_n, 1);
+      s_key[slot] = v;
+      s_idx[slot] = vox;
+    }
   }
 }
 
 __device__ __forceinline__ bool before3(float ka, int ia, float kb, int ib) { return (ka > kb) || (ka == kb && ia < ib); }
 
-__global__ void __launch_bounds__(1024) bev_top64_kernel(const int* __restrict__ cand_count, const int* __restrict__ cand_idx,
+// One CTA per frame: bitonic sort of the frame's candidates (value desc, index asc), the first 64 out.  A frame with more
+// than kCandCap maxima sorts the exact top 64 of select64 instead of its truncated candidate list.
+__global__ void __launch_bounds__(1024) bev_top64_kernel(const float* __restrict__ c3d, const uint32_t* __restrict__ max_mask,
+                                                         const int* __restrict__ cand_count, const int* __restrict__ cand_idx,
                                                          const float* __restrict__ cand_val, int* __restrict__ counts,
                                                          int* __restrict__ top_idx, float* __restrict__ top_val) {
   __shared__ float s_key[kCandCap];
   __shared__ int s_idx[kCandCap];
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int n = min(cand_count[b], kCandCap);
+  const bool overflow = cand_count[b] > kCandCap;
+  const int n = overflow ? kMaxP : cand_count[b];
   for (int i = tid; i < kCandCap; i += 1024) {
-    s_key[i] = i < n ? cand_val[(size_t)b * kCandCap + i] : -CUDART_INF_F;
-    s_idx[i] = i < n ? cand_idx[(size_t)b * kCandCap + i] : 0x7fffffff;
+    s_key[i] = i < n && !overflow ? cand_val[(size_t)b * kCandCap + i] : -CUDART_INF_F;
+    s_idx[i] = i < n && !overflow ? cand_idx[(size_t)b * kCandCap + i] : 0x7fffffff;
   }
   __syncthreads();
+  if (overflow) {
+    select64(c3d + (size_t)b * kVol, max_mask + (size_t)b * (kVol / 32), s_key, s_idx);
+    __syncthreads();
+  }
   for (int k = 2; k <= kCandCap; k <<= 1)
     for (int j = k >> 1; j > 0; j >>= 1) {
       for (int t = tid; t < kCandCap / 2; t += 1024) {
@@ -831,7 +905,7 @@ int b200romp_bev_center3d(b200romp_bev* h, const float* maps_fv, const void* bv_
 }
 
 long long b200romp_bev_parse_workspace_bytes(int batch) {
-  return (long long)batch * (sizeof(int) * 2 + kCandCap * 8 + kMaxP * 8);
+  return (long long)batch * (sizeof(int) * 2 + kCandCap * 8 + kMaxP * 8 + kVol / 8);
 }
 
 int b200romp_bev_parse3d(const float* center3d, int batch, float thresh, int capacity, int* d_count, long long* batch_ids,
@@ -845,10 +919,11 @@ int b200romp_bev_parse3d(const float* center3d, int batch, float thresh, int cap
   float* cand_val = reinterpret_cast<float*>(cand_idx + (size_t)batch * kCandCap);
   int* top_idx = reinterpret_cast<int*>(cand_val + (size_t)batch * kCandCap);
   float* top_val = reinterpret_cast<float*>(top_idx + (size_t)batch * kMaxP);
+  uint32_t* max_mask = reinterpret_cast<uint32_t*>(top_val + (size_t)batch * kMaxP);
   B2R_CUDA_OK(cudaMemsetAsync(cand_count, 0, sizeof(int) * batch, stream));
-  const size_t n = (size_t)batch * kVol;
-  bev_nms3d_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(center3d, batch, thresh, cand_count, cand_idx, cand_val);
-  bev_top64_kernel<<<batch, 1024, 0, stream>>>(cand_count, cand_idx, cand_val, counts, top_idx, top_val);
+  static_assert(kVol % 256 == 0, "bev_nms3d_kernel: one thread per voxel, whole CTAs and warps per frame");
+  bev_nms3d_kernel<<<(unsigned)((size_t)batch * kVol / 256), 256, 0, stream>>>(center3d, thresh, cand_count, cand_idx, cand_val, max_mask);
+  bev_top64_kernel<<<batch, 1024, 0, stream>>>(center3d, max_mask, cand_count, cand_idx, cand_val, counts, top_idx, top_val);
   bev_emit_kernel<<<batch, 64, 0, stream>>>(batch, capacity, counts, top_idx, top_val, d_count, batch_ids, czyx, conf);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;

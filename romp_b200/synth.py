@@ -438,6 +438,14 @@ def bev_state_dict(seed: int = 0, gain: float = 0.55):
     return sd
 
 
+def bev_noise_volume(seed: int):
+    """One 3-D centre-map frame [1,64,128,128] of noise in [0.1, 0.2) with every value distinct (a random permutation of
+    an even grid whose step exceeds the fp32 spacing there): about 8,800 local maxima (5x5x5) above 0.08, so the top-64
+    of the parse is defined without a tie rule."""
+    n = 64 * 128 * 128
+    return (0.1 + 0.1 * np.random.RandomState(seed).permutation(n) / n).astype(np.float32).reshape(1, 64, 128, 128)
+
+
 # --------------------------------------------------------------------------------------
 # ResNet-50 backbone variant of ROMP (workload cfg1; romp/lib/models/resnet_50.py:19-120)
 # --------------------------------------------------------------------------------------

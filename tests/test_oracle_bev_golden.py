@@ -44,6 +44,18 @@ def test_bev_maps_and_model(golden_dir):
     assert np.abs(B.cam_to_trans(pk["cam"]).numpy() - zp["cam_trans"]).max() < 1e-5
 
 
+def test_parse_3d_dense_noise(golden_dir):
+    """More than 4,096 local maxima in one frame: the oracle's top-64 (value desc, index asc) is the reference's own."""
+    z = g(golden_dir, "bev_parse_dense.npz")
+    vol = synth.bev_noise_volume(int(z["seed"]))
+    bi, czyx, conf = B.parse_3d(vol, float(z["thresh"]))
+    assert int(z["n_maxima"]) > 4096 and len(bi) == 64
+    assert np.array_equal(bi.numpy(), z["batch_ids"])
+    assert np.array_equal(czyx.numpy(), z["czyx"])
+    assert np.array_equal(conf.numpy(), z["conf"])
+    assert np.array_equal(conf.numpy(), vol[0][tuple(z["czyx"].T)])
+
+
 def test_bev_post(golden_dir):
     z = g(golden_dir, "bev_post.npz")
     pack_a, pack_s = synth.smpl_pack(0, num_betas=11), synth.smpl_pack(1)
