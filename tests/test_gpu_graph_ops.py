@@ -1,46 +1,61 @@
 """Every op of the shipped conv graphs, checked in place against a float64 reference computed from its own inputs.
 
-Graphs and batches:
-  - ROMP bf16 with u8 frames (graph.build_romp) at batch 64, the benchmarked configuration;
-  - ROMP TF32 with u8 frames at batch 34;
-  - BEV bf16 G1 at batch 34 and G2 (the bird's-eye Conv1d stack) at batch 136.
+Graphs and batches (all with u8 frames):
+  - ROMP bf16 (graph.build_romp) at batch 64, the benchmarked configuration; ROMP TF32 at batch 34; ROMP fp32 (the SIMT
+    engine) at batch 5;
+  - ROMP with the ResNet-50 backbone (graph.build_romp_resnet50, --backbone resnet50): bf16 at batch 64 (the CLI
+    default), TF32 at batch 34, fp32 at batch 5;
+  - BEV G1 and G2 (the bird's-eye Conv1d stack): bf16 at batches 34 and 136, TF32 at 34 and 16, fp32 at 5 and 16 (G2 runs
+    on the SIMT engine outside bf16).
 A persistent tensor-core kernel loops over tiles, so a scheduling bug can hide in the third tile a CTA runs (the fused block
 kernel flips its mbarrier parity every tile).  The batches are picked so that the ops reach that tile where one graph fits
 comfortably on the device; an op that needs more than 2 x 132 / tiles-per-frame frames for it (the unmerged 1x1 256->32
 fuse conv of the last HRNet stage, 2 tiles per 16x16 frame on 132 CTAs) is run once more on its own, with its recorded
 weights and its real input frames repeated, at a batch that gives some CTA 3 tiles (133).  The describe() plan of that
-rerun must equal the graph's.
+rerun must equal the graph's.  A fused Bottleneck cannot run alone: the graph batch itself must give it 3 tiles (layer1
+of both backbones has 128 tiles per frame).  The fp32 graphs have no persistent kernels, so they run at a small batch.
 
 How an op is checked:
   1. The builder's library calls (add_tensor, add_const_tensor, add_conv, add_sum, add_maxpool, set_lane, finalize) are
      recorded through a proxy of the loaded library while the builder runs.
   2. The recorded graph is replayed with one maxpool "keeper" per internal tensor appended before finalize, so the buffer
      planner recycles nothing and every op's input, residual, sum terms and output survive the run.  A fused block's
-     intermediate gets no keeper (a second reader would undo the fusion).  The keeper net's op lines must equal the
-     production net's: same engines, plans, pixel-pair folds, block fusions and grids.
+     intermediate gets no keeper (a second reader would undo the fusion); a fused Bottleneck's two do, and the kernel
+     then also stores them, so each of its three describe() lines is checked as a conv of its own.  The keepers are known
+     by their output tensors (the ResNet-50 graph has a maxpool of its own).  The keeper net's op lines must equal the
+     production net's: same engines, plans, pixel-pair folds, block and Bottleneck fusions and grids.
   3. After one run, each op is recomputed in float64 with torch on the GPU from the tensors it read, and every element of
      its output slice must lie within
          bf16 out: 2^-8 |v| + g A,   fp32 out: 2^-23 |v| + g A,   g = 2^-24 (K + 3),
      with v the float64 result, A the same op on |X|, |W|, |b|, |res| and K the reduction length.  The operands are those
      the engine multiplies: bf16 weights as recorded, TF32-rounded activations and weights on the tc-tf32 engine, the
-     stem engine's bf16(w * 2/255).  A fused block's reference intermediate is bf16(relu(conv1 + b1)), zero outside the
-     frame; where conv1's float64 value lies within g A1 of a bf16 rounding midpoint the kernel may round the other way,
-     so conv(|W2|, one ulp + g A1) is added there.  A sum is bounded by 2^-8 |v| + 2^-24 (n + 1) sum|terms|, 1.1**z by
-     carrying z's bound through the power.
+     stem engine's bf16(w * 2/255).  ConvTranspose2d(4, 2, 1) is referenced by F.conv_transpose2d with K = 4 cin (2 x 2
+     taps per input channel reach each output); the ResNet-50 7x7 stem multiplies the raw u8 values (the recorded weights
+     carry the normalisation) and adds its one-frame fp32 bias map to every frame.  A fused block's reference
+     intermediate is bf16(relu(conv1 + b1)), zero outside the frame; where conv1's float64 value lies within g A1 of a
+     bf16 rounding midpoint the kernel may round the other way, so conv(|W2|, one ulp + g A1) is added there.  A sum is
+     bounded by 2^-8 |v| + 2^-24 (n + 1) sum|terms|, 1.1**z by carrying z's bound through the power.  A maxpool is exact:
+     it must equal the float64 max_pool2d(3, 2, padding 1) with -inf padding bit for bit.
   Output slices are checked after the whole run: a later op that writes into an earlier op's slice fails the check.
-Negative controls mutate the reference of a few ops (one dropped tap, one dropped bias, a residual taken from the
-neighbouring channel pair) and must be rejected; test_bound_calibration_cpu runs the same bound on the CPU against an
-fp32 implementation with another summation order.
+Negative controls mutate the reference of a few ops (one dropped tap of a conv, block, transposed conv or 7x7 stem, one
+dropped bias, a residual taken from the neighbouring channel pair, a maxpool window shifted by one pixel) and must be
+rejected; test_bound_calibration_cpu runs the same bound on the CPU against an fp32 implementation with another
+summation order.
 
-Whole-graph checks compare bits: production net (buffer reuse) vs keeper net, each frame at batch 64 vs batch 1 and inside
-a batch of 7, CUDA graph vs eager launches, concurrency lanes vs one stream, and more than 16 distinct (frames, output)
-bindings, which clears the CUDA-graph cache (for G2: changes of the bv_in pointer and of the batch, on which the Conv1d
-tensor map is re-encoded).
+Whole-graph checks compare bits: production net (buffer reuse) vs keeper net for every graph; in bf16 also each frame at
+batch 64 vs batch 1 and inside a batch of 7; for HRNet bf16 CUDA graph vs eager launches, concurrency lanes vs one stream,
+and more than 16 distinct (frames, output) bindings, which clears the CUDA-graph cache (for G2: changes of the bv_in
+pointer and of the batch, on which the Conv1d tensor map is re-encoded); for ResNet-50 bf16 u8 frames vs fp32 frames
+holding the same integers.
 
-Measured on one H100 80GB HBM3 (torch's peak allocation plus the keeper net's workspace; weights not counted), with the
+Measured on one H100 80GB HBM3 at a 700 W power limit (torch's peak allocation plus the keeper net's workspace; weights not counted), with the
 runtime of each test including the whole-graph checks:
-  ROMP bf16, batch 64: 12.0 GiB (9.8 GiB keeper workspace), 10 s;   ROMP TF32, batch 34: 15.4 GiB, 4 s;
-  BEV G1, batch 34: 7.8 GiB;  G2, batch 136: 1.2 GiB;  BEV test 4.5 s.
+  ROMP bf16, batch 64: 12.0 GiB (9.8 GiB keeper workspace), 10-14 s;   ROMP TF32, batch 34: 15.4 GiB, 4 s;
+  ROMP fp32, batch 5: 2.6 GiB, 2 s;
+  ROMP ResNet-50 bf16, batch 64: 9.8 GiB (7.6 GiB keeper workspace), 7 s;   TF32, batch 34: 9.8 GiB, 4 s;
+  ROMP ResNet-50 fp32, batch 5: 1.8 GiB, 2 s;
+  BEV bf16 G1, batch 34: 7.8 GiB;  G2, batch 136: 1.2 GiB;  test 4.5-5.3 s;
+  BEV TF32 G1, batch 34: 16.9 GiB;  G2, batch 16: 0.9 GiB;  test 5 s;   BEV fp32 G1, batch 5: 2.8 GiB;  G2: 0.3 GiB;  2 s.
 """
 import ctypes as C
 import math
@@ -73,16 +88,27 @@ def _nchw(t):
     return t.permute(0, 3, 1, 2)
 
 
-def conv_bound(x, w, b, *, stride=1, relu=False, res=None, up=1, pow_channel=-1, out_dt=BF16, input_norm=0):
+def conv_bound(x, w, b, *, stride=1, relu=False, res=None, up=1, pow_channel=-1, out_dt=BF16, input_norm=0, transpose=False):
     """float64 result v and per-element bound of one conv op; x, res: NHWC float64 (res may have one frame), w, b float64
-    tensors.  input_norm: x holds raw 0..255 values; the kernel's normalised fp32 input carries 2^-22 absolute error."""
-    K = w.shape[1] * (w.shape[2] * (w.shape[3] if w.ndim == 4 else 1))
+    tensors.  input_norm: x holds raw 0..255 values; the kernel's normalised fp32 input carries 2^-22 absolute error.
+    transpose: ConvTranspose2d(4, 2, 1) with w in PyTorch's [cin, cout, 4, 4] layout; each output sums 2 x 2 taps per
+    input channel, so K = 4 cin."""
     if input_norm:
         x = x / 255.0 * 2.0 - 1.0
-    kw = dict(stride=stride, up=up, device=x.device, dtype=torch.float64)
-    z = conv_ref(x, w, b, **kw)
+    if transpose:
+        K = 4 * w.shape[0]
+
+        def ref(x_, w_, b_):
+            return F.conv_transpose2d(_nchw(x_), w_, b_, stride=2, padding=1).permute(0, 2, 3, 1)
+    else:
+        K = w.shape[1] * (w.shape[2] * (w.shape[3] if w.ndim == 4 else 1))
+        kw = dict(stride=stride, up=up, device=x.device, dtype=torch.float64)
+
+        def ref(x_, w_, b_):
+            return conv_ref(x_, w_, b_, **kw)
+    z = ref(x, w, b)
     ax = x.abs() + (2.0 ** -22 if input_norm else 0.0)
-    A = conv_ref(ax, w.abs(), None if b is None else b.abs(), **kw)
+    A = ref(ax, w.abs(), None if b is None else b.abs())
     if res is not None:
         z = z + res
         A = A + res.abs()
@@ -137,6 +163,13 @@ def sum_bound(base, terms, ups, relu, out_dt):
     if relu:
         v = v.clamp_min(0)
     return v, ROUND[out_dt] * v.abs() + 2.0 ** -24 * (len(terms) + 1) * a
+
+
+def maxpool_ref(x, shift=0):
+    """MaxPool2d(3, 2, padding 1) of NHWC float64 x with -inf padding (a max is exact: no bound); shift moves every
+    window `shift` pixels down and right"""
+    xp = F.pad(_nchw(x), (1 - shift, 1 + shift, 1 - shift, 1 + shift), value=-math.inf)
+    return F.max_pool2d(xp, 3, 2).permute(0, 2, 3, 1)
 
 
 def excess(got, v, bound):
@@ -307,11 +340,14 @@ class Net:
 # ---------------------------------------------------------------------------------------------------------------------
 TC_RE = re.compile(r"\[tc(-tf32)? k(\d) v(\d) nt(\d+) grid (\d+)x(\d+) smem \d+ stages \d+( pixel-pairs)?\]")
 BLOCK_RE = re.compile(r"mid t(\d+).*\[tc-block grid (\d+) smem \d+( conv1 pixel-pairs conv2 pixel-pairs)?\]")
+BOTTLENECK_RE = re.compile(r"\[tc-bottleneck conv(\d) of k1-k3-k1 grid (\d+) smem \d+\]")
 IO_RE = re.compile(r" in t(\d+)\[.*? out t(\d+)\[")
+OUT_RE = re.compile(r" out t(\d+)\[")
 
 
 def ops_of(record, lines):
-    """pair each op line of the production describe() with its recorded call(s)"""
+    """pair each op line of the production describe() with its recorded call(s); a fused Bottleneck prints one line per
+    conv, each paired with that conv's call"""
     calls = [c for c in record["calls"] if c[0] in ("conv", "sum", "maxpool")]
     ops, i = [], 0
     for line in lines:
@@ -328,15 +364,23 @@ def ops_of(record, lines):
         if c[0] == "sum":
             ops.append(dict(line=line, kind="sum", sum=c[2][0]))
             continue
+        io = IO_RE.search(line)
+        io = (int(io.group(1)), int(io.group(2)))
+        if c[0] == "maxpool":
+            assert " maxpool " in line and io == c[2], line
+            ops.append(dict(line=line, kind="maxpool", io=c[2]))
+            continue
         assert c[0] == "conv", line
         d = c[2][0]
-        io = IO_RE.search(line)
-        assert (int(io.group(1)), int(io.group(2))) == (d.in_, d.out), line
+        assert io == (d.in_, d.out), line
         op = dict(line=line, kind="conv", conv=c[2], tc=None)
         m = TC_RE.search(line)
         if m:
             op["tc"] = dict(tf32=bool(m.group(1)), k=int(m.group(2)), v=int(m.group(3)), grid=int(m.group(5)),
                             fold=bool(m.group(7)), bracket=m.group(0))
+        m = BOTTLENECK_RE.search(line)
+        if m:
+            op["tc"] = dict(bottleneck=int(m.group(1)), tf32=False, grid=int(m.group(2)), fold=False, bracket=m.group(0))
         ops.append(op)
     assert i == len(calls), "describe() has fewer op lines than the recorded graph"
     return ops
@@ -345,11 +389,13 @@ def ops_of(record, lines):
 def op_class(op):
     if op["kind"] == "block":
         return "folded block" if op["fold"] else "block"
-    if op["kind"] == "sum":
-        return "sum"
+    if op["kind"] in ("sum", "maxpool"):
+        return op["kind"]
     d, tc = op["conv"][0], op["tc"]
-    if tc is None:
-        return "SIMT"
+    if tc is None:       # the CUDA-core kernels: ConvTranspose2d(4, 2, 1), the 7x7 stem, the SIMT engine
+        return {42: "deconv", 7: "k7"}.get(d.ksize, "SIMT")
+    if "bottleneck" in tc:
+        return "bottleneck"
     if tc["v"] == 3:
         return "conv1d" if d.ksize == 13 else "stem"
     if d.stride == 2:
@@ -396,6 +442,19 @@ def check_op(op, read, batch, frames=None, mutate=None):
         v, bnd = sum_bound(base.double(), [t.double() for t in terms], ups, bool(s.relu), _dt(out_t))
         r, o = excess(out_t, v, bnd)
         return r, o, nz_in, bool((out_t != 0).any())
+    if op["kind"] == "maxpool":
+        x_all, out_all = read(op["io"][0]), read(op["io"][1])
+        shift = [0]
+        if mutate:
+            mutate("maxpool", shift)
+        nz_in = float((x_all != 0).float().mean())
+        step = max(1, CHUNK // (x_all[0].numel() * 2))
+        idx = list(sel)
+        for i in range(0, len(idx), step):
+            fr = idx[i:i + step]
+            v = maxpool_ref(x_all[fr].double(), shift[0]).to(out_all.dtype).double()   # exact: must equal bit for bit
+            over += int((out_all[fr].double() != v).sum())
+        return (math.inf if over else 0.0), over, nz_in, bool((out_all != 0).any())
     if op["kind"] == "block":
         (d1, w1, b1), (d2, w2, b2) = op["convs"]
         Cc = d1.cin
@@ -418,7 +477,8 @@ def check_op(op, read, batch, frames=None, mutate=None):
         return worst, over, nz_in, bool((y_all != 0).any())
     d, w, b = op["conv"]
     tc = op["tc"]
-    shape = (d.cout, d.cin, 3) if d.ksize == 13 else (d.cout, d.cin, d.ksize, d.ksize)
+    transpose = d.ksize == 42          # ConvTranspose2d(4, 2, 1): PyTorch's [cin, cout, 4, 4] weights
+    shape = (d.cout, d.cin, 3) if d.ksize == 13 else (d.cin, d.cout, 4, 4) if transpose else (d.cout, d.cin, d.ksize, d.ksize)
     wt = torch.from_numpy(w.reshape(shape)).cuda()
     bt = None if b is None else torch.from_numpy(b).cuda().double()
     x_all = read(d.in_)
@@ -430,7 +490,7 @@ def check_op(op, read, batch, frames=None, mutate=None):
     wt = wt.double()
     x_all = x_all[..., d.in_c_off:d.in_c_off + d.cin]
     if mutate:
-        mutate("conv", [wt, bt], x_all.double().abs().mean((0, 1, 2)))
+        mutate("deconv" if transpose else "conv", [wt, bt], x_all.double().abs().mean((0, 1, 2)))
     out_all = read(d.out)[..., d.out_c_off:d.out_c_off + d.cout]
     res_all = None if d.res < 0 else read(d.res)[..., d.res_c_off:d.res_c_off + d.cout]
     if res_all is not None and mutate:
@@ -447,7 +507,7 @@ def check_op(op, read, batch, frames=None, mutate=None):
         if res_all is not None:
             res = res_all[:1].double() if d.res_broadcast else res_all[fr].double()
         v, bnd = conv_bound(x, wt, bt, stride=d.stride, relu=bool(d.relu), res=res, up=d.upsample, pow_channel=d.pow_channel,
-                            out_dt=_dt(out_all), input_norm=d.input_norm)
+                            out_dt=_dt(out_all), input_norm=d.input_norm, transpose=transpose)
         r, o = excess(out_all[fr], v, bnd)
         worst, over = max(worst, r), over + o
     return worst, over, nz_in, bool((out_all != 0).any())
@@ -482,10 +542,10 @@ class Reader:
 def internal_tensors(r, mids):
     written = set()
     for kind, _, args in r["calls"]:
-        if kind == "conv":
+        if kind in ("conv", "sum"):
             written.add(args[0].out)
-        elif kind == "sum":
-            written.add(args[0].out)
+        elif kind == "maxpool":
+            written.add(args[1])
     return [t for t, s in r["tensors"].items()
             if t in written and not s["ext"] and not s["const"] and not s["nchw"] and t not in mids]
 
@@ -509,8 +569,11 @@ def keeper_net(r, prod_lines):
     keep = internal_tensors(r, mids)
     net = Net.replay(r, keep=keep)
     lines = net.op_lines()
-    body = [l for l in lines if " maxpool " not in l]
+    # the keepers are the ops replay appended: known by their output tensors (the graph may have maxpools of its own)
+    kept_out = set(net.keepers)
+    body = [l for l in lines if int(OUT_RE.search(l).group(1)) not in kept_out]
     assert len(lines) - len(body) == len(keep)
+    assert all(int(OUT_RE.search(l).group(1)) in kept_out for l in lines[len(body):]), "a keeper is not last"
     assert body == prod_lines, "the keepers changed a kernel choice:\n" + "\n".join(
         f"{a}\n{b}" for a, b in zip(body, prod_lines) if a != b)
     return net
@@ -610,7 +673,9 @@ def verify_graph(name, r, prod_lines, batch, inputs, report):
             few_tiles.append(op)
     reruns = []
     for op in few_tiles:
-        assert op["kind"] == "conv", op["line"]
+        # a fused op cannot run alone: its graph batch must give it 3 tiles on some CTA
+        assert op["kind"] == "conv" and op_class(op) != "bottleneck", \
+            f"{name}: fused op below 3 tiles per CTA at batch {batch}:\n{op['line']}"
         B, tiles, worst, over = rerun_alone(op, read, batch)
         read.keep_only(())
         reruns.append((op_class(op), op["line"].split(" [")[0], B, tiles, worst))
@@ -642,17 +707,25 @@ def verify_graph(name, r, prod_lines, batch, inputs, report):
 # negative controls: the comparison must reject a wrong reference
 # ---------------------------------------------------------------------------------------------------------------------
 def drop_tap(which=0):
-    """zero the tap of output channel 5 of the weight array `which` (0 = conv1 of a block) that contributes most: largest
-    |w| times the mean |input| of its channel (synthetic weights leave some channels dead after a ReLU)"""
+    """zero the tap of one output channel of the weight array `which` (0 = conv1 of a block) that contributes most: largest
+    |w| times the mean |input| of its channel.  Synthetic weights leave some channels dead after a ReLU, so with the mean
+    |input| known the output channel is the one of largest mean pre-activation sum(w * mean|input|) + b, else channel 5."""
     def f(kind, a, act=None):
-        if kind not in ("conv", "block"):
+        if kind not in ("conv", "block", "deconv"):
             return
-        w = a[0] if kind == "conv" else a[2 * which]
-        flat = w[5].reshape(-1)
-        score = w[5].abs()
-        if act is not None and which == 0:
-            score = score * act.reshape((-1,) + (1,) * (w.ndim - 2))
-        flat[score.reshape(-1).argmax()] = 0
+        i = 2 * which if kind == "block" else 0
+        w, b = a[i], a[i + 1]
+        if kind == "deconv":      # [cin, cout, 4, 4] -> a [cout, cin, 4, 4] view
+            w = w.transpose(0, 1)
+        co = 5
+        score = w[co].abs()
+        if act is not None and i == 0:
+            act = act.reshape((-1,) + (1,) * (w.ndim - 2))
+            pre = (w * act).flatten(1).sum(1) + (0 if b is None else b)
+            co = int(pre.argmax())
+            score = w[co].abs() * act
+        taps = w[co]
+        taps[torch.unravel_index(score.argmax(), score.shape)] = 0
     return f
 
 
@@ -671,17 +744,33 @@ def swap_res_pair(ch):
     return f
 
 
+def shift_window():
+    """every maxpool window of the reference one pixel down and right: it starts at 2 oy instead of 2 oy - 1"""
+    def f(kind, a, act=None):
+        if kind == "maxpool":
+            a[0] = 1
+    return f
+
+
 def negative_controls(ops, read, batch, report):
     """each mutation of the reference must be rejected by the bound"""
     def first(pred):
         return next(op for op in ops if pred(op))
 
     tries = []
-    if any(op_class(op) == "folded block" for op in ops):
-        tries.append(("folded 32-channel block, one tap", first(lambda o: op_class(o) == "folded block"), drop_tap()))
-    if any(op_class(op) == "block" for op in ops):
-        tries.append(("64-channel block, one tap", first(lambda o: op_class(o) == "block"), drop_tap()))
-    tries.append(("stride-2 conv, one tap", first(lambda o: op_class(o) == "s2"), drop_tap()))
+    for cls, what, mut in (("folded block", "folded 32-channel block, one tap", drop_tap()),
+                           ("block", "64-channel block, one tap", drop_tap()),
+                           ("k7", "7x7 stem, one tap", drop_tap()),
+                           ("maxpool", "maxpool, window shifted by one pixel", shift_window())):
+        if any(op_class(op) == cls for op in ops):
+            tries.append((what, first(lambda o: op_class(o) == cls), mut))
+    deconvs = [op for op in ops if op_class(op) == "deconv"]
+    if deconvs:     # the shortest reduction: one of the 8192 taps of the 2048-channel one is within 2^-24 (K + 3) A
+        tries.append(("transposed conv, one tap", min(deconvs, key=lambda o: o["conv"][0].cin), drop_tap()))
+    # by descriptor, on any engine: a stride-2 1x1 or 3x3 conv of activations (not the u8 stem)
+    tries.append(("stride-2 conv, one tap", first(lambda o: o["kind"] == "conv" and o["conv"][0].stride == 2 and
+                                                  o["conv"][0].ksize in (1, 3) and
+                                                  read.net.tensors[o["conv"][0].in_]["dt"] != U8), drop_tap()))
     heads = [op for op in ops if op["kind"] == "conv" and read.net.tensors[op["conv"][0].out]["nchw"]]
     if heads:
         tries.append(("head output conv, its largest bias", heads[-1], drop_bias()))
@@ -692,7 +781,7 @@ def negative_controls(ops, read, batch, report):
     for what, op, mut in tries:
         worst, over, _, _ = check_op(op, read, batch, frames=frames, mutate=mut)
         read.keep_only(())
-        report(f"   negative control {what}: {over} elements over the bound (worst ratio {worst:.1f}) -> rejected")
+        report(f"   negative control {what}: {over} elements over the bound (worst ratio {worst:.3g}) -> rejected")
         assert over > 0, f"negative control not rejected: {what} on\n{op['line']}"
 
 
@@ -707,6 +796,11 @@ def romp_sd():
 @pytest.fixture(scope="module")
 def bev_sd():
     return synth.bev_state_dict(0)
+
+
+@pytest.fixture(scope="module")
+def resnet50_sd():
+    return synth.resnet50_state_dict(0)
 
 
 def _say(s):
@@ -734,8 +828,20 @@ def _builder_net(nb, r):
     return Net(_lib.load(), nb.net, dict(r["tensors"]), r["max_batch"])
 
 
+def _check_batch_invariance(prod, io, keys, frames, kept, stream):
+    """frame i alone and inside a batch of 7 gives the bits of frame i of the full batch"""
+    batch = frames.shape[0]
+    for i in (0, batch // 2 - 1, batch - 1):
+        one = _outputs(prod, io, keys, 1, frames[i:i + 1].contiguous(), stream)
+        lo = min(max(i - 3, 0), batch - 7)
+        seven = _outputs(prod, io, keys, 7, frames[lo:lo + 7].contiguous(), stream)
+        for k in keys:
+            assert torch.equal(one[k][0], kept[k][i]), f"{k}: frame {i} at batch 1 differs from batch {batch}"
+            assert torch.equal(seven[k][i - lo], kept[k][i]), f"{k}: frame {i} in a batch of 7 differs"
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision,batch", [("bf16", 64), ("tf32", 34)])
+@pytest.mark.parametrize("precision,batch", [("bf16", 64), ("tf32", 34), ("fp32", 5)])
 def test_romp_graph_ops(monkeypatch, romp_sd, precision, batch):
     t0 = time.time()
     torch.cuda.synchronize()
@@ -755,14 +861,7 @@ def test_romp_graph_ops(monkeypatch, romp_sd, precision, batch):
     for k in keys:
         assert torch.equal(outs[k], kept[k]), f"{k}: production net differs from the keeper net"
     if precision == "bf16":
-        # batch invariance: frame i alone and inside a batch of 7 equals frame i of the full batch
-        for i in (0, batch // 2 - 1, batch - 1):
-            one = _outputs(prod, io, keys, 1, frames[i:i + 1].contiguous(), stream)
-            lo = min(max(i - 3, 0), batch - 7)
-            seven = _outputs(prod, io, keys, 7, frames[lo:lo + 7].contiguous(), stream)
-            for k in keys:
-                assert torch.equal(one[k][0], kept[k][i]), f"{k}: frame {i} at batch 1 differs from batch {batch}"
-                assert torch.equal(seven[k][i - lo], kept[k][i]), f"{k}: frame {i} in a batch of 7 differs"
+        _check_batch_invariance(prod, io, keys, frames, kept, stream)
         # the CUDA-graph cache holds 16 bindings: 18 distinct (frames, output) buffers make it clear itself
         alive = []                       # every binding stays allocated: no address repeats
         for j in range(18):
@@ -785,31 +884,73 @@ def test_romp_graph_ops(monkeypatch, romp_sd, precision, batch):
     _say(f"   ROMP {precision}: total {time.time() - t0:.1f} s")
 
 
-BEV_G1_BATCH, BEV_G2_BATCH = 34, 136
-
-
 @pytest.mark.gpu
-def test_bev_graph_ops(monkeypatch, bev_sd):
+@pytest.mark.parametrize("precision,batch", [("bf16", 64), ("tf32", 34), ("fp32", 5)])
+def test_romp_resnet50_graph_ops(monkeypatch, resnet50_sd, precision, batch):
+    """ROMP with the ResNet-50 backbone (--backbone resnet50): the 7x7 stem on raw u8 frames, MaxPool2d(3, 2, 1), the
+    1x1 convs to 512 / 1024 channels, the fused Bottlenecks of layer1 (bf16), the K-split 256-channel stride-2 conv of
+    layer3.0, the SIMT convs of 512..2048 input channels and the three ConvTranspose2d(4, 2, 1)."""
     t0 = time.time()
-    (g1, io1, g2, io2), (r1, r2) = record(monkeypatch, lambda: graph.build_bev(bev_sd, 0, "bf16", U8, BEV_G1_BATCH),
-                                         finalize_batch={1: BEV_G2_BATCH})
+    torch.cuda.synchronize()
+    (nb, io), (r,) = record(monkeypatch, lambda: graph.build_romp_resnet50(resnet50_sd, 0, precision, U8, batch))
+    prod = _builder_net(nb, r)
+    frames = _frames(batch, seed=51)
+    name = f"ROMP ResNet-50 {precision}"
+    net, binds, ops, stream, read = verify_graph(name, r, prod.op_lines(), batch, {io["frames"]: frames}, _say)
+    classes = {op_class(op) for op in ops}
+    assert {"k7", "maxpool", "deconv", "SIMT"} <= classes, classes
+    assert precision != "bf16" or "bottleneck" in classes, classes
+    negative_controls(ops, read, batch, _say)
+    keys = ("center_maps", "params_maps")
+    kept = {k: binds[io[k]] for k in keys}
+    net.destroy()
+    read.cache.clear()
+
+    outs = _outputs(prod, io, keys, batch, frames, stream)
+    for k in keys:
+        assert torch.equal(outs[k], kept[k]), f"{k}: production net differs from the keeper net"
+    if precision == "bf16":
+        _check_batch_invariance(prod, io, keys, frames, kept, stream)
+        # the stem multiplies raw values: fp32 frames holding the same integers give the same bits as u8 frames
+        nbf, iof = graph.build_romp_resnet50(resnet50_sd, 0, precision, F32, 8)
+        other = _builder_net(nbf, r)
+        got = _outputs(other, iof, keys, 8, frames[:8].float(), stream)
+        other.destroy()
+        for k in keys:
+            assert torch.equal(got[k], kept[k][:8]), f"{k}: fp32 frames differ from u8 frames"
+    prod.destroy()
+    _say(f"   {name}: total {time.time() - t0:.1f} s")
+
+
+# G1 at batch 34 takes every tensor-core op but one (see the module docstring) to 3 tiles per CTA, in bf16 and TF32 alike;
+# the fp32 graphs are SIMT only, and G2 outside bf16 is too.
+BEV_BATCHES = {"bf16": (34, 136), "tf32": (34, 16), "fp32": (5, 16)}
+
+
+def _bev_graph_ops(monkeypatch, bev_sd, precision):
+    """BEV's G1 and G2 at `precision`: every op checked, negative controls on G1, production vs keeper net, G2 bindings"""
+    t0 = time.time()
+    b1, b2 = BEV_BATCHES[precision]
+    (g1, io1, g2, io2), (r1, r2) = record(monkeypatch, lambda: graph.build_bev(bev_sd, 0, precision, U8, b1),
+                                         finalize_batch={1: b2})
     p1, p2 = _builder_net(g1, r1), _builder_net(g2, r2)
-    frames = _frames(BEV_G1_BATCH, seed=33)
+    frames = _frames(b1, seed=33)
     keys1 = ("maps_fv", "fv_feats", "img_feats")
-    net1, binds1, ops1, stream, read1 = verify_graph("BEV G1", r1, p1.op_lines(), BEV_G1_BATCH, {io1["frames"]: frames}, _say)
-    negative_controls(ops1, read1, BEV_G1_BATCH, _say)
+    net1, binds1, ops1, stream, read1 = verify_graph(f"BEV {precision} G1", r1, p1.op_lines(), b1,
+                                                     {io1["frames"]: frames}, _say)
+    negative_controls(ops1, read1, b1, _say)
     kept1 = {k: binds1[io1[k]] for k in keys1}
     net1.destroy()
     read1.cache.clear()
-    outs = _outputs(p1, io1, keys1, BEV_G1_BATCH, frames, stream)
+    outs = _outputs(p1, io1, keys1, b1, frames, stream)
     for k in keys1:
         assert torch.equal(outs[k], kept1[k]), f"{k}: production G1 differs from the keeper net"
     p1.destroy()
 
     # G2 on a non-negative bird's-eye input (it is assembled from ReLU features)
     g = torch.Generator(device="cuda").manual_seed(7)
-    bv = torch.randn(BEV_G2_BATCH, 1, 128, 2560, generator=g, device="cuda").abs().bfloat16()
-    net2, binds2, ops2, stream, read2 = verify_graph("BEV G2", r2, p2.op_lines(), BEV_G2_BATCH, {io2["bv_in"]: bv}, _say)
+    bv = torch.randn(b2, 1, 128, 2560, generator=g, device="cuda").abs().to(TD[r2["tensors"][io2["bv_in"]]["dt"]])
+    net2, binds2, ops2, stream, read2 = verify_graph(f"BEV {precision} G2", r2, p2.op_lines(), b2, {io2["bv_in"]: bv}, _say)
     kept2 = binds2[io2["bv_out"]]
     net2.destroy()
     read2.cache.clear()
@@ -821,30 +962,47 @@ def test_bev_graph_ops(monkeypatch, bev_sd):
         stream.synchronize()
         return out
 
-    assert torch.equal(g2_run(bv, BEV_G2_BATCH), kept2), "bv_out: production G2 differs from the keeper net"
+    assert torch.equal(g2_run(bv, b2), kept2), "bv_out: production G2 differs from the keeper net"
     # the Conv1d tensor map is re-encoded when bv_in moves or the batch changes: 18 bindings of varying batch
     alive = []
     for j in range(18):
         n = 1 + (j * 5) % 9
-        lo = (j * 7) % (BEV_G2_BATCH - n)
+        lo = (j * 7) % (b2 - n)
         alive.append(bv[lo:lo + n].clone())
         alive.append(g2_run(alive[-1], n))
         assert torch.equal(alive[-1], kept2[lo:lo + n]), f"bv_out: binding {j} (batch {n})"
     p2.destroy()
-    _say(f"   BEV: total {time.time() - t0:.1f} s")
+    _say(f"   BEV {precision}: total {time.time() - t0:.1f} s")
+
+
+@pytest.mark.gpu
+def test_bev_graph_ops(monkeypatch, bev_sd):
+    _bev_graph_ops(monkeypatch, bev_sd, "bf16")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["tf32", "fp32"])
+def test_bev_graph_ops_fp32_tensors(monkeypatch, bev_sd, precision):
+    """BEV with fp32 activations: G1 on the TF32 engine (16 image-feature channels on the SIMT engine) or the SIMT
+    engine, G2 on the SIMT engine"""
+    _bev_graph_ops(monkeypatch, bev_sd, precision)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # the bound itself, on the CPU
 # ---------------------------------------------------------------------------------------------------------------------
-def _alt_conv(x, w, b, stride, res, relu, parts=4):
-    """another implementation: fp32 torch on the CPU, K split into channel groups summed in reverse order, bf16 output"""
-    cin = w.shape[1]
+def _alt_conv(x, w, b, stride, res, relu, parts=4, transpose=False):
+    """another implementation: fp32 torch on the CPU, K split into channel groups summed in reverse order, bf16 output.
+    transpose: ConvTranspose2d(4, 2, 1) with w [cin, cout, 4, 4]; a one-frame residual is broadcast over the batch."""
+    cin = w.shape[0 if transpose else 1]
     step = max(1, cin // parts)
     acc = None
     for c0 in reversed(range(0, cin, step)):
-        y = F.conv2d(_nchw(x[..., c0:c0 + step]).float(), w[:, c0:c0 + step].float(), None, stride=stride,
-                     padding=w.shape[-1] // 2)
+        xs = _nchw(x[..., c0:c0 + step]).float()
+        if transpose:
+            y = F.conv_transpose2d(xs, w[c0:c0 + step].float(), None, stride=2, padding=1)
+        else:
+            y = F.conv2d(xs, w[:, c0:c0 + step].float(), None, stride=stride, padding=w.shape[-1] // 2)
         acc = y if acc is None else acc + y
     acc = acc + b.float()[None, :, None, None]
     if res is not None:
@@ -855,19 +1013,34 @@ def _alt_conv(x, w, b, stride, res, relu, parts=4):
 
 
 @pytest.mark.parametrize("k,cin,cout,stride,hw,res", [(3, 64, 64, 1, 16, True), (3, 32, 32, 1, 32, True), (1, 256, 32, 1, 8, False),
-                                                       (3, 32, 64, 2, 32, False), (1, 64, 256, 1, 16, True)])
+                                                       (3, 32, 64, 2, 32, False), (1, 64, 256, 1, 16, True),
+                                                       (42, 64, 32, 2, 8, False), (7, 3, 64, 2, 32, "broadcast")])
 def test_bound_calibration_cpu(k, cin, cout, stride, hw, res):
     """The per-element bound accepts a legitimate other implementation of the same op and rejects the mutations the GPU
-    negative controls use: a dropped tap, a dropped bias, a residual from the neighbouring channel pair."""
+    negative controls use: a dropped tap, a dropped bias, a residual from the neighbouring channel pair.
+    k = 42 is ConvTranspose2d(4, 2, 1) (weights [cin, cout, 4, 4]); the 7x7 case is the ResNet-50 stem: raw u8 values
+    times weights scaled by 1 / (255 std), plus a one-frame fp32 residual broadcast over the batch."""
     g = torch.Generator().manual_seed(k * 100 + cin + cout)
-    x = torch.randn(3, hw, hw, cin, generator=g).clamp_min(0).bfloat16()
-    w = (torch.randn(cout, cin, k, k, generator=g) / math.sqrt(cin * k * k)).bfloat16().double()
+    transpose = k == 42
+    if k == 7:
+        x = torch.randint(0, 256, (3, hw, hw, cin), generator=g, dtype=torch.uint8)
+        w = (torch.randn(cout, cin, k, k, generator=g) / math.sqrt(cin * k * k) / 57.0).bfloat16().double()
+    elif transpose:
+        x = torch.randn(3, hw, hw, cin, generator=g).clamp_min(0).bfloat16()
+        w = (torch.randn(cin, cout, 4, 4, generator=g) / math.sqrt(4 * cin)).double()
+    else:
+        x = torch.randn(3, hw, hw, cin, generator=g).clamp_min(0).bfloat16()
+        w = (torch.randn(cout, cin, k, k, generator=g) / math.sqrt(cin * k * k)).bfloat16().double()
     b = 0.1 * torch.randn(cout, generator=g, dtype=torch.float64)
-    ho = hw // stride
-    r = torch.randn(3, ho, ho, cout, generator=g).bfloat16() if res else None
-    got = _alt_conv(x, w, b, stride, r, relu=True)
+    ho = 2 * hw if transpose else hw // stride
+    if res == "broadcast":
+        r = torch.randn(1, ho, ho, cout, generator=g)
+    else:
+        r = torch.randn(3, ho, ho, cout, generator=g).bfloat16() if res else None
+    got = _alt_conv(x, w, b, stride, r, relu=True, transpose=transpose)
     rd = None if r is None else r.double()
-    v, bnd = conv_bound(x.double(), w, b, stride=stride, relu=True, res=rd)
+    kw = dict(stride=stride, relu=True, transpose=transpose)
+    v, bnd = conv_bound(x.double(), w, b, res=rd, **kw)
     worst, over = excess(got, v, bnd)
     print(f"k{k} s{stride} {cin}->{cout}: fp32 CPU implementation worst |err|/bound {worst:.3f}")
     assert over == 0 and worst < 1
@@ -875,14 +1048,14 @@ def test_bound_calibration_cpu(k, cin, cout, stride, hw, res):
     w2 = w.clone()
     flat = w2[5].reshape(-1)
     flat[flat.abs().argmax()] = 0
-    assert excess(got, *conv_bound(x.double(), w2, b, stride=stride, relu=True, res=rd))[1] > 0, "dropped tap accepted"
+    assert excess(got, *conv_bound(x.double(), w2, b, res=rd, **kw))[1] > 0, "dropped tap accepted"
     b2 = b.clone()
     b2[b.abs().argmax()] = 0
-    assert excess(got, *conv_bound(x.double(), w, b2, stride=stride, relu=True, res=rd))[1] > 0, "dropped bias accepted"
+    assert excess(got, *conv_bound(x.double(), w, b2, res=rd, **kw))[1] > 0, "dropped bias accepted"
     if res:
         r2 = rd.clone()
         r2[..., 2:4] = rd[..., 4:6]
-        assert excess(got, *conv_bound(x.double(), w, b, stride=stride, relu=True, res=r2))[1] > 0, "swapped residual accepted"
+        assert excess(got, *conv_bound(x.double(), w, b, res=r2, **kw))[1] > 0, "swapped residual accepted"
 
 
 @pytest.mark.parametrize("cin", [32, 64])
