@@ -8,25 +8,37 @@
 // FOLD = true runs a 32-channel block on the pixel-pair view [B, H, W/2, 64] with the folded 64x64 weights of
 // net.cu fold_pixel_pairs; the all-zero tap halves are skipped at compile time.
 //
-// Geometry, per 16x8 output tile at (y0, x0) of frame n (pixel pairs when folded):
-//   input stage: ONE TMA load of the 20x12 halo at (x0-2, y0-2), channels innermost, 128 B swizzle, zeros outside the
-//            frame.  Halo pixel (hy, hx) is stage row hy*12 + hx.
-//   conv1:   over a LINEAR domain: mid pixel (my, mx), my < 18, mx < 10, is GEMM row my*12 + mx, so tap (r, s) is the stage
-//            shifted by r*12 + s rows and the 8-row groups are contiguous (SBO = 1024 B).  Rows 0..213 are needed, padded to
-//            256 (4 m64 blocks): warpgroup g computes rows 128g..128g+127.  Columns 10, 11 of a mid row and rows >= 214 are
-//            never read by conv2; the stage rows 240..281 TMA never writes feed only those.
+// Geometry, per 16 x TW output tile at (y0, x0) of frame n (pixel pairs when folded); TW = 8 for C = 64, 16 folded, and
+// HW = TW + 4 the halo width:
+//   input stage: ONE TMA load of the 20 x HW halo at (x0-2, y0-2), channels innermost, 128 B swizzle, zeros outside the
+//            frame.  Halo pixel (hy, hx) is stage row hy*HW + hx.
+//   conv1:   over a LINEAR domain: mid pixel (my, mx), my < 18, mx < TW + 2, is GEMM row my*HW + mx, so tap (r, s) is the
+//            stage shifted by r*HW + s rows and the 8-row groups are contiguous (SBO = 1024 B).  Rows up to 17*HW + TW + 1 are
+//            needed (213 / 357), padded to whole m64 blocks (4 / 6): warpgroup g computes the second half of them, in passes
+//            of at most two blocks.  Columns >= TW + 2 of a mid row and the padding rows are never read by conv2; the stage
+//            rows TMA never writes (from 20*HW on) feed only those.
 //   mid:     relu(acc + b1) -> bf16, zero where the mid pixel lies outside the frame (the unfused conv2 reads TMA zero fill
-//            there), stored to a 256 x 128 B buffer in the swizzled layout wgmma reads (16 B chunk ^ (row & 7)).
-//   conv2:   the conv_tc.cu 3x3 mapping on the mid buffer: 8-pixel groups, SBO = 12 rows, tap (r, s) shifted by r*12 + s
-//            rows.  Warpgroup g computes output tile rows 8g..8g+7 (one m64 x N = 64).
+//            there), stored to the mid buffer in the swizzled layout wgmma reads (16 B chunk ^ (row & 7)).
+//   conv2:   the conv_tc.cu 3x3 mapping on the mid buffer: 8-pixel groups, SBO = HW rows, tap (r, s) shifted by r*HW + s
+//            rows.  Warpgroup g computes output tile rows 8g..8g+7, one m64 x N = 64 per 8 columns.
 //   output:  (acc + b2) + x, ReLU, bf16.  x at the output pixels is the interior of the halo: read from shared memory
 //            before the stage is handed back.
 // Both convs keep the K order of conv_tc_kernel (taps 0..8 x 32-byte k-steps, the same folded halves skipped), so the fp32
 // sums and therefore t and y are bit-identical to the unfused path.
 //
-// Shared memory: both convs' weights stay resident (2 x 72 KB), next to ONE input stage (36 KB) and the mid buffer (32 KB):
-// 212 KB of the 227 KB.  With room for one stage only, both consumer warpgroups work on the same tile; the stage goes back to
-// the producer once conv1 has retired, so the next tile's TMA load overlaps the mid epilogue, conv2 and the output epilogue.
+// Shared memory: both convs' weights stay resident next to ONE input stage and the mid buffer.  A 64-channel conv takes
+// 72 KB: with a 16x8 tile (36 KB stage, 32 KB mid) that is 212 KB of the 227 KB.  The folded weights hold only the halves
+// the MMAs read: the three s = 0 taps as full 64 x 128 B tiles (128 B swizzle), the six s = -1 / s = +1 taps as 64 x 64 B
+// tiles of the 32 input channels they use (64 B swizzle, w_tap_off), so a folded conv takes 48 KB.  The freed room holds a
+// 16x16 tile (54 KB stage, 48 KB mid; 200 KB in all): conv1 computes 384 rows for 256 outputs instead of 256 for 128, so
+// a folded block issues 240 MMAs per 256 output pixel pairs instead of 288, and the per-tile fixed costs (barriers,
+// pipeline drains, the halo's two extra columns) are spread over twice the pixels.  With one stage both consumer
+// warpgroups work on the same tile; the stage goes back to the producer once conv1 has retired, so the next tile's TMA
+// load overlaps the mid epilogue, conv2 and the output epilogue.
+// A folded variant that kept the 16x8 tile, spent the freed 48 KB on a second input stage and issued conv1 of tile j + 1
+// right after conv2 of tile j (so it ran through tile j's output epilogue) measured 155.4 us per block against 154.5 us
+// (H100 80GB HBM3, 700 W, batch 64 at 128^2), so it was not kept: hiding the output epilogue is not what the remaining gap
+// to the operand-fetch bound is made of.
 #include "conv_tc.cuh"
 #include "tc_device.cuh"
 
@@ -36,20 +48,48 @@ namespace {
 
 constexpr int kBlkThreads = 384;                        // warp 0 = TMA producer, warpgroups 1, 2 = consumers
 constexpr int kRowB = 128;                              // one pixel row: 64 bf16 channels = one 128 B swizzle span
-constexpr int kHaloW = 12, kHaloH = 20;                 // input halo of a 16x8 output tile, two 3x3 convs deep
+constexpr int kHaloH = 20;                              // input halo of a 16-row output tile, two 3x3 convs deep
 constexpr int kTapBytes = 64 * kRowB;                   // one tap of one conv: 64 output x 64 input channels
-constexpr int kWBytes = 9 * kTapBytes;
-constexpr int kStagePayload = kHaloH * kHaloW * kRowB;  // what TMA writes: 240 rows
-constexpr int kStageBytes = (282 * kRowB + 1023) / 1024 * 1024;   // + the rows 240..281 the padded mid rows read
-constexpr int kMidBytes = 256 * kRowB;
-constexpr int kSmemBytes = 2 * kWBytes + kStageBytes + kMidBytes + 1024 /*barriers*/ + 1024 /*align slack*/;
-static_assert(kSmemBytes <= 227 * 1024, "fused block does not fit shared memory");
+constexpr int kHalfTapBytes = 64 * 64;                  // the used half of a folded s = -1 / +1 tap: 64 x 32, 64 B rows
+
+template <bool FOLD>
+struct BlkCfg {
+  static constexpr int kWBytes = FOLD ? 3 * (kTapBytes + 2 * kHalfTapBytes) : 9 * kTapBytes;   // per conv
+  static constexpr int kTW = FOLD ? 16 : 8;                 // output tile width; the height is 16
+  static constexpr int kHaloW = kTW + 4;
+  static constexpr int kBPW = FOLD ? 3 : 2;                 // conv1 m64 blocks per warpgroup
+  static constexpr int kC2 = kTW / 8;                       // conv2 m64 blocks per warpgroup (8-column groups)
+  static constexpr int kMidRows = 2 * kBPW * 64;
+  static constexpr int kStagePayload = kHaloH * kHaloW * kRowB;                                   // what TMA writes
+  static constexpr int kStageBytes = ((kMidRows + 2 * kHaloW + 2) * kRowB + 1023) / 1024 * 1024;  // + what padded rows read
+  static constexpr int kMidBytes = kMidRows * kRowB;
+  static constexpr int kSmemBytes = 2 * kWBytes + kStageBytes + kMidBytes + 1024 /*barriers*/ + 1024 /*align slack*/;
+  static_assert(17 * kHaloW + kTW + 1 < kMidRows, "conv1 blocks do not cover the mid pixels conv2 reads");
+  static_assert(kHaloH * kHaloW - 2 * kHaloW - 2 > 17 * kHaloW + kTW + 1, "an unwritten stage row feeds a mid row conv2 reads");
+  static_assert(kSmemBytes <= 227 * 1024, "fused block does not fit shared memory");
+  static_assert(kWBytes % kTapBytes == 0, "weights are copied in tap-sized pieces");
+};
+
+// byte offset of tap `tap` in a conv's weight image.  Folded, each kernel row r holds [s = -1 half | s = 0 full | s = +1 half]
+// in 16 KB, so every full tile starts 1024 B-aligned (128 B swizzle) and every half tile 512 B-aligned (64 B swizzle).
+__host__ __device__ constexpr int w_tap_off(bool fold, int tap) {
+  return !fold ? tap * kTapBytes
+               : (tap / 3) * (kTapBytes + 2 * kHalfTapBytes) + (tap % 3 == 0 ? 0 : tap % 3 == 1 ? kHalfTapBytes : kHalfTapBytes + kTapBytes);
+}
 
 // the MMAs of a pixel-pair folded conv that only meet all-zero weights: first pixel (k-steps 0, 1) of the s = -1 taps,
 // second pixel (k-steps 2, 3) of the s = +1 taps (net.cu fold_pixel_pairs, the kmask of the unfused path)
 template <bool FOLD>
 __device__ __forceinline__ constexpr bool blk_skip(int tap, int k) {
   return FOLD && ((tap % 3 == 0 && k < 2) || (tap % 3 == 2 && k >= 2));
+}
+
+// B descriptor of k-step k of tap `tap` (k not skipped): a half tile holds the two k-steps its tap reads
+template <bool FOLD>
+__device__ __forceinline__ uint64_t w_desc(uint32_t w_base, int tap, int k) {
+  const uint32_t t = w_base + (uint32_t)w_tap_off(FOLD, tap);
+  if (FOLD && tap % 3 != 1) return make_smem_desc(t + (k & 1) * 32, 8 * 64, kSw64);
+  return make_smem_desc(t + k * 32, 8 * kRowB, kSw128);
 }
 
 // barrier over both consumer warpgroups (id 1; 0 is __syncthreads)
@@ -76,19 +116,149 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&v);
 }
 
+// one consumer thread: warpgroup g, warp w of it, lane l, and its channel pair cl inside each 8-channel group
+struct BlkThread {
+  int g, w, l, cl;
+};
+struct BlkTile {
+  int n, y0, x0;
+  __device__ BlkTile(int tile, int tiles_x, int per_frame, int tw) {
+    n = tile / per_frame;
+    const int rem = tile % per_frame;
+    y0 = (rem / tiles_x) * 16;
+    x0 = (rem % tiles_x) * tw;
+  }
+};
+
+// conv1 over the stage at a_base: NB m64 blocks of mid rows from row0.  Issued and committed as one group.
+template <bool FOLD, int NB>
+__device__ __forceinline__ void conv1_issue(float (&acc)[2][32], uint32_t a_base, uint32_t w1_base, int row0) {
+  constexpr int kHaloW = BlkCfg<FOLD>::kHaloW;
+#pragma unroll
+  for (int h = 0; h < NB; ++h)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
+  uint32_t scale_d = 0;
+  wgmma_fence();
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap) {
+    const uint32_t a_tap = a_base + (uint32_t)((row0 + (tap / 3) * kHaloW + tap % 3) * kRowB);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (blk_skip<FOLD>(tap, k)) continue;
+      const uint64_t bdesc = w_desc<FOLD>(w1_base, tap, k);
+#pragma unroll
+      for (int h = 0; h < NB; ++h)
+        wgmma_n64(acc[h], make_smem_desc(a_tap + h * 64 * kRowB + k * 32, 8 * kRowB, kSw128), bdesc, scale_d, false);
+      scale_d = 1;
+    }
+  }
+  wgmma_commit();
+}
+
+// residual = the block input at this thread's output pixels (tile row 8g + 2w + e, column 8c + l / 4): halo pixel
+// (row + 2, column + 2) of the stage at a_base
+template <bool FOLD>
+__device__ __forceinline__ void load_residual(uint32_t (&rv)[BlkCfg<FOLD>::kC2][2][8], uint32_t a_base, const BlkThread& th) {
+  constexpr int kHaloW = BlkCfg<FOLD>::kHaloW;
+#pragma unroll
+  for (int c = 0; c < BlkCfg<FOLD>::kC2; ++c)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int hr = (8 * th.g + 2 * th.w + e + 2) * kHaloW + 8 * c + (th.l >> 2) + 2;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) rv[c][e][j] = ld_shared_b32(a_base + hr * kRowB + ((j ^ (hr & 7)) << 4) + 2 * th.cl);
+    }
+}
+
+// relu(acc + b1), zero where the mid pixel lies outside the frame (the unfused conv2 reads TMA zero fill there), bf16,
+// stored to the mid buffer in the swizzled layout wgmma reads (16 B chunk ^ (row & 7))
+template <bool FOLD, int NB>
+__device__ __forceinline__ void mid_epilogue(const float (&acc)[2][32], uint32_t mid_base, const float* b1p, const ConvParams& p,
+                                             const BlkTile& tl, const BlkThread& th, int row0) {
+  constexpr int kHaloW = BlkCfg<FOLD>::kHaloW;
+#pragma unroll
+  for (int h = 0; h < NB; ++h) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int m = row0 + 64 * h + 16 * th.w + (th.l >> 2) + 8 * e;
+      const int my = m / kHaloW, mx = m % kHaloW;
+      const bool inside = my < 18 && mx < BlkCfg<FOLD>::kTW + 2 && (unsigned)(tl.y0 - 1 + my) < (unsigned)p.Hout && (unsigned)(tl.x0 - 1 + mx) < (unsigned)p.Wout;
+      const uint32_t row = mid_base + m * kRowB;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + th.cl;
+        float a = fmaxf(acc[h][4 * j + 2 * e] + __ldg(b1p + c), 0.f);
+        float b = fmaxf(acc[h][4 * j + 2 * e + 1] + __ldg(b1p + c + 1), 0.f);
+        if (!inside) a = b = 0.f;
+        st_shared_b32(row + ((j ^ (m & 7)) << 4) + 2 * th.cl, pack_bf16x2(a, b));
+      }
+    }
+  }
+}
+
+// conv2 over the mid buffer: output tile rows 8g .. 8g + 7, one m64 per 8-column group.  Issued and committed as one group.
+template <bool FOLD>
+__device__ __forceinline__ void conv2_issue(float (&acc2)[BlkCfg<FOLD>::kC2][32], uint32_t mid_base, uint32_t w2_base, int g) {
+  constexpr int kHaloW = BlkCfg<FOLD>::kHaloW, kC2 = BlkCfg<FOLD>::kC2;
+#pragma unroll
+  for (int c = 0; c < kC2; ++c)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc2[c][j] = 0.f;
+  uint32_t scale_d = 0;
+  wgmma_fence();
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap) {
+    const uint32_t a_tap = mid_base + (uint32_t)(((8 * g + tap / 3) * kHaloW + tap % 3) * kRowB);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (blk_skip<FOLD>(tap, k)) continue;
+      const uint64_t bdesc = w_desc<FOLD>(w2_base, tap, k);
+#pragma unroll
+      for (int c = 0; c < kC2; ++c)
+        wgmma_n64(acc2[c], make_smem_desc(a_tap + 8 * c * kRowB + k * 32, kHaloW * kRowB, kSw128), bdesc, scale_d, false);
+      scale_d = 1;
+    }
+  }
+  wgmma_commit();
+}
+
+// (acc + b2) + x, ReLU, bf16 (the order of the unfused conv2)
+template <bool FOLD>
+__device__ __forceinline__ void out_epilogue(const float (&acc2)[BlkCfg<FOLD>::kC2][32], const uint32_t (&rv)[BlkCfg<FOLD>::kC2][2][8],
+                                             const float* b2p, const ConvParams& p, const BlkTile& tl, const BlkThread& th) {
+  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
+#pragma unroll
+  for (int q = 0; q < 2 * BlkCfg<FOLD>::kC2; ++q) {
+    const int c = q >> 1, e = q & 1;
+    const size_t pix = ((size_t)tl.n * p.Hout + tl.y0 + 8 * th.g + 2 * th.w + e) * p.Wout + tl.x0 + 8 * c + (th.l >> 2);
+    __nv_bfloat162* o = reinterpret_cast<__nv_bfloat162*>(out + pix * p.out_C + p.out_c_off + th.cl);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int ch = 8 * j + th.cl;
+      float a = acc2[c][4 * j + 2 * e] + __ldg(b2p + ch), b = acc2[c][4 * j + 2 * e + 1] + __ldg(b2p + ch + 1);
+      const float2 r = res_pair(rv[c][e][j]);
+      a += r.x; b += r.y;
+      o[4 * j] = __floats2bfloat162_rn(fmaxf(a, 0.f), fmaxf(b, 0.f));
+    }
+  }
+}
+
 }  // namespace
 
 template <bool FOLD>
 __global__ void __launch_bounds__(kBlkThreads, 1)
 conv_block_tc_kernel(const __grid_constant__ CUtensorMap tmap, const ConvParams p, const uint8_t* __restrict__ w1pack,
                      const uint8_t* __restrict__ w2pack, const float* __restrict__ bias1, int tiles_x, int tiles_y, int num_tiles) {
+  using Cfg = BlkCfg<FOLD>;
+  constexpr int kWBytes = Cfg::kWBytes, kStageBytes = Cfg::kStageBytes, kBPW = Cfg::kBPW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sW1 = smem;
   uint8_t* sW2 = smem + kWBytes;
   uint8_t* sA = smem + 2 * kWBytes;
   uint8_t* sMid = sA + kStageBytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sMid + kMidBytes);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sMid + Cfg::kMidBytes);
   uint64_t* empty = full + 1;
   uint64_t* w_full = full + 2;
 
@@ -107,130 +277,54 @@ conv_block_tc_kernel(const __grid_constant__ CUtensorMap tmap, const ConvParams 
     // ===================== TMA producer =====================
     if (elect_one()) {
       mbar_arrive_expect_tx(w_full, 2 * kWBytes);
-      for (int t = 0; t < 9; ++t) {
-        bulk_copy_g2s(sW1 + t * kTapBytes, w1pack + (size_t)t * kTapBytes, kTapBytes, w_full);
-        bulk_copy_g2s(sW2 + t * kTapBytes, w2pack + (size_t)t * kTapBytes, kTapBytes, w_full);
+      for (int off = 0; off < kWBytes; off += kTapBytes) {
+        bulk_copy_g2s(sW1 + off, w1pack + off, kTapBytes, w_full);
+        bulk_copy_g2s(sW2 + off, w2pack + off, kTapBytes, w_full);
       }
       pdl_wait();                             // weights are constants; activations must wait for the predecessor grids
       const uint64_t pol = l2_policy_stream();
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, phase ^= 1) {
-        const int n = tile / per_frame, rem = tile % per_frame;
-        const int y0 = (rem / tiles_x) * 16, x0 = (rem % tiles_x) * 8;
+        const BlkTile tl(tile, tiles_x, per_frame, Cfg::kTW);
         mbar_wait(empty, phase ^ 1);
-        mbar_arrive_expect_tx(full, kStagePayload);
-        tma_load_4d(sA, &tmap, full, 0, x0 - 2, y0 - 2, n, pol);
+        mbar_arrive_expect_tx(full, Cfg::kStagePayload);
+        tma_load_4d(sA, &tmap, full, 0, tl.x0 - 2, tl.y0 - 2, tl.n, pol);
       }
     }
   } else if (warp >= 4) {
     // ===================== consumers: both warpgroups work on every tile of the CTA =====================
-    const int g = (warp >> 2) - 1, t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    const int t = threadIdx.x & 127;
+    const BlkThread th{(warp >> 2) - 1, t >> 5, t & 31, 2 * (t & 3)};
     pdl_wait();                               // output writes must follow the predecessor grids
     mbar_wait(w_full, 0);
-    const int cl = 2 * (l & 3);               // this thread's channel pair inside each 8-channel group
+    float acc[2][32], acc2[Cfg::kC2][32];
+    uint32_t rv[Cfg::kC2][2][8];
+    const int row0 = th.g * kBPW * 64;          // this warpgroup's first conv1 row
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, phase ^= 1) {
       const uint32_t w1_base = opaque(smem_u32(sW1)), w2_base = opaque(smem_u32(sW2)), a_base = opaque(smem_u32(sA)),
                      mid_base = opaque(smem_u32(sMid));
       const float* b1p = opaque(bias1);
       const float* b2p = opaque(p.bias);
-      const int n = tile / per_frame, rem = tile % per_frame;
-      const int y0 = (rem / tiles_x) * 16, x0 = (rem % tiles_x) * 8;
+      const BlkTile tl(tile, tiles_x, per_frame, Cfg::kTW);
       mbar_wait(full, phase);
-
-      // ---- conv1: mid rows 128g .. 128g + 127 as two m64 blocks
-      float acc[2][32];
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
-      uint32_t scale_d = 0;
-      wgmma_fence();
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        const uint32_t a_tap = a_base + (uint32_t)((128 * g + (tap / 3) * kHaloW + tap % 3) * kRowB);
-        const uint32_t b_tap = w1_base + (uint32_t)(tap * kTapBytes);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          if (blk_skip<FOLD>(tap, k)) continue;
-          const uint64_t bdesc = make_smem_desc(b_tap + k * 32, 8 * kRowB, kSw128);
-          wgmma_n64(acc[0], make_smem_desc(a_tap + k * 32, 8 * kRowB, kSw128), bdesc, scale_d, false);
-          wgmma_n64(acc[1], make_smem_desc(a_tap + 64 * kRowB + k * 32, 8 * kRowB, kSw128), bdesc, scale_d, false);
-          scale_d = 1;
-        }
-      }
-      wgmma_commit();
-      // residual = the block input at this thread's output pixels (tile row 8g + 2w + e, column l / 4): halo pixel
-      // (row + 2, column + 2), loaded while the MMAs run
-      uint32_t rv[2][8];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int hr = (8 * g + 2 * w + e + 2) * kHaloW + (l >> 2) + 2;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) rv[e][j] = ld_shared_b32(a_base + hr * kRowB + ((j ^ (hr & 7)) << 4) + 2 * cl);
-      }
+      conv1_issue<FOLD, 2>(acc, a_base, w1_base, row0);
+      load_residual<FOLD>(rv, a_base, th);    // while the MMAs run
       wgmma_wait<0>();
-      mbar_arrive(empty);                     // the stage goes back to the producer: the next tile's load overlaps the rest
-
-      // ---- mid epilogue: relu(acc + b1), zero outside the frame, bf16, swizzled into the mid buffer
+      if constexpr (kBPW == 2) mbar_arrive(empty);   // the stage goes back to the producer: the next tile's load overlaps the rest
       consumers_bar_sync();                   // both warpgroups' conv2 of the previous tile has retired
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int m = 64 * (2 * g + h) + 16 * w + (l >> 2) + 8 * e;
-          const int my = m / kHaloW, mx = m % kHaloW;
-          const bool inside = my < 18 && mx < 10 && (unsigned)(y0 - 1 + my) < (unsigned)p.Hout && (unsigned)(x0 - 1 + mx) < (unsigned)p.Wout;
-          const uint32_t row = mid_base + m * kRowB;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int c = 8 * j + cl;
-            float a = fmaxf(acc[h][4 * j + 2 * e] + __ldg(b1p + c), 0.f);
-            float b = fmaxf(acc[h][4 * j + 2 * e + 1] + __ldg(b1p + c + 1), 0.f);
-            if (!inside) a = b = 0.f;
-            st_shared_b32(row + ((j ^ (m & 7)) << 4) + 2 * cl, pack_bf16x2(a, b));
-          }
-        }
+      mid_epilogue<FOLD, 2>(acc, mid_base, b1p, p, tl, th, row0);
+      if constexpr (kBPW == 3) {              // the third block of this warpgroup's conv1 rows
+        conv1_issue<FOLD, 1>(acc, a_base, w1_base, row0 + 128);
+        wgmma_wait<0>();
+        mbar_arrive(empty);
+        mid_epilogue<FOLD, 1>(acc, mid_base, b1p, p, tl, th, row0 + 128);
       }
       fence_proxy_async();                    // generic-proxy stores -> visible to wgmma
       consumers_bar_sync();
-
-      // ---- conv2: output tile rows 8g .. 8g + 7
-      float acc2[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc2[j] = 0.f;
-      scale_d = 0;
-      wgmma_fence();
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        const uint32_t a_tap = mid_base + (uint32_t)(((8 * g + tap / 3) * kHaloW + tap % 3) * kRowB);
-        const uint32_t b_tap = w2_base + (uint32_t)(tap * kTapBytes);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          if (blk_skip<FOLD>(tap, k)) continue;
-          wgmma_n64(acc2, make_smem_desc(a_tap + k * 32, kHaloW * kRowB, kSw128), make_smem_desc(b_tap + k * 32, 8 * kRowB, kSw128),
-                    scale_d, false);
-          scale_d = 1;
-        }
-      }
-      wgmma_commit();
+      conv2_issue<FOLD>(acc2, mid_base, w2_base, th.g);
       wgmma_wait<0>();
-
-      // ---- output epilogue: (acc + b2) + x, ReLU, bf16 (the order of the unfused conv2)
-      __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const size_t pix = ((size_t)n * p.Hout + y0 + 8 * g + 2 * w + e) * p.Wout + x0 + (l >> 2);
-        __nv_bfloat162* o = reinterpret_cast<__nv_bfloat162*>(out + pix * p.out_C + p.out_c_off + cl);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int c = 8 * j + cl;
-          float a = acc2[4 * j + 2 * e] + __ldg(b2p + c), b = acc2[4 * j + 2 * e + 1] + __ldg(b2p + c + 1);
-          const float2 r = res_pair(rv[e][j]);
-          a += r.x; b += r.y;
-          o[4 * j] = __floats2bfloat162_rn(fmaxf(a, 0.f), fmaxf(b, 0.f));
-        }
-      }
+      out_epilogue<FOLD>(acc2, rv, b2p, p, tl, th);
     }
   }
 }
@@ -238,14 +332,30 @@ conv_block_tc_kernel(const __grid_constant__ CUtensorMap tmap, const ConvParams 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-bool tc_block_supported(const ConvParams& p) {
+bool tc_block_supported(const ConvParams& p, bool fold) {
   if (p.in_dtype != B200ROMP_BF16 || p.out_dtype != B200ROMP_BF16 || p.res_dtype != B200ROMP_BF16) return false;
   if (p.cin != 64 || p.cout != 64 || p.up != 1 || p.out_nchw || p.pow_channel >= 0 || p.input_norm || !p.relu) return false;
-  if (p.Hin != p.Hout || p.Win != p.Wout || p.Hout % 16 != 0 || p.Wout % 8 != 0) return false;
+  if (p.Hin != p.Hout || p.Win != p.Wout || p.Hout % 16 != 0 || p.Wout % (fold ? BlkCfg<true>::kTW : BlkCfg<false>::kTW) != 0) return false;
   if (p.in_C % 8 != 0 || p.in_c_off % 8 != 0 || p.out_C % 8 != 0 || p.out_c_off % 8 != 0) return false;
   // the residual is read from the staged input halo: it must be the block's input slice itself
   if (p.res != p.in || p.res_C != p.in_C || p.res_c_off != p.in_c_off || p.res_broadcast) return false;
   return (reinterpret_cast<uintptr_t>(p.in) & 15) == 0;
+}
+
+// one conv's weight image in shared-memory order.  Folded: the s = 0 taps as 128 B-row tiles, and of each s = -1 / s = +1
+// tap only the 64 B-row chunk of the input channels its MMAs read (channels 32..63 = the second pixel of the pair for
+// s = -1, channels 0..31 = the first for s = +1), at w_tap_off.
+static int block_pack_weights(const float* w_oihw, bool fold, void** d_out, std::vector<void*>* allocs) {
+  if (!fold) return tc_pack_weights(w_oihw, 64, 64, 9, 64, d_out, allocs, kRowB, 2);
+  const std::vector<uint8_t> full = tc_pack_image(w_oihw, 64, 64, 9, 64, kRowB, 2);   // [tap][64 x 128 B]
+  const std::vector<uint8_t> half = tc_pack_image(w_oihw, 64, 64, 9, 64, 64, 2);      // [tap][chunk][64 x 64 B]
+  std::vector<uint8_t> img(BlkCfg<true>::kWBytes);
+  for (int tap = 0; tap < 9; ++tap) {
+    uint8_t* dst = img.data() + w_tap_off(true, tap);
+    if (tap % 3 == 1) memcpy(dst, full.data() + (size_t)tap * kTapBytes, kTapBytes);
+    else memcpy(dst, half.data() + (size_t)(2 * tap + (tap % 3 == 0 ? 1 : 0)) * kHalfTapBytes, kHalfTapBytes);
+  }
+  return tc_upload_image(img, d_out, allocs);
 }
 
 int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
@@ -261,21 +371,21 @@ int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1,
   plan->grid_x = sm_count;
   plan->grid_y = 1;
   plan->stages = 1;
-  plan->smem_bytes = kSmemBytes;
-  int rc = tc_pack_weights(w1_oihw, 64, 64, 9, 64, &plan->d_wpack, allocs, kRowB, 2);
+  plan->smem_bytes = plan->fold ? BlkCfg<true>::kSmemBytes : BlkCfg<false>::kSmemBytes;
+  int rc = block_pack_weights(w1_oihw, plan->fold, &plan->d_wpack, allocs);
   if (rc) return rc;
-  rc = tc_pack_weights(w2_oihw, 64, 64, 9, 64, &plan->d_wpack2, allocs, kRowB, 2);
+  rc = block_pack_weights(w2_oihw, plan->fold, &plan->d_wpack2, allocs);
   if (rc) return rc;
   void* db1 = nullptr;
   B2R_CUDA_OK(cudaMalloc(&db1, 64 * sizeof(float)));
   allocs->push_back(db1);
   B2R_CUDA_OK(cudaMemcpy(db1, b1, 64 * sizeof(float), cudaMemcpyHostToDevice));
   plan->d_bias1 = static_cast<const float*>(db1);
-  // tensor map over the NHWC input slice: dims (C, W, H, N), 20x12 halo box, OOB -> zeros
+  // tensor map over the NHWC input slice: dims (C, W, H, N), 20 x (TW + 4) halo box, OOB -> zeros
   CUtensorMap tm;
   const cuuint64_t gdim[4] = {64, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
   const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * 2, (cuuint64_t)p.Win * p.in_C * 2, (cuuint64_t)p.Hin * p.Win * p.in_C * 2};
-  const cuuint32_t box[4] = {64, kHaloW, kHaloH, 1};
+  const cuuint32_t box[4] = {64, (cuuint32_t)(plan->fold ? BlkCfg<true>::kHaloW : BlkCfg<false>::kHaloW), kHaloH, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * 2);
   CUresult cr = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -285,15 +395,15 @@ int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1,
     return B200ROMP_ECUDA;
   }
   memcpy(plan->tmap_in, &tm, sizeof(tm));
-  B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+  B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BlkCfg<false>::kSmemBytes));
+  B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BlkCfg<true>::kSmemBytes));
   return B200ROMP_OK;
 }
 
 int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) {
   CUtensorMap tm;
   memcpy(&tm, plan.tmap_in, sizeof(tm));
-  const int tiles_x = p.Wout / 8, tiles_y = p.Hout / 16;
+  const int tiles_x = p.Wout / (plan.fold ? BlkCfg<true>::kTW : BlkCfg<false>::kTW), tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   const dim3 grid(std::min(plan.grid_x, num_tiles));
   auto kern = plan.fold ? conv_block_tc_kernel<true> : conv_block_tc_kernel<false>;

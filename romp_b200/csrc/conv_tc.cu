@@ -236,7 +236,7 @@ float tc_round_tf32_host(float w) {
   return r;
 }
 
-int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, void** d_out, std::vector<void*>* allocs, int rowb, int eb) {
+std::vector<uint8_t> tc_pack_image(const float* w_oihw, int cin, int cout, int taps, int nt, int rowb, int eb) {
   // shared-memory image [n-tile][tap][chunk][NT rows x rowb bytes] with the TMA/wgmma XOR swizzle; elements bf16 (eb = 2)
   // or fp32 rounded to TF32 (eb = 4)
   const int cw = rowb / eb, kch = cin / cw, ntiles = (cout + nt - 1) / nt, per16 = 16 / eb;
@@ -257,10 +257,18 @@ int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, vo
             else { const float f = tc_round_tf32_host(w); memcpy(tile + byte, &f, 4); }
           }
       }
+  return img;
+}
+
+int tc_upload_image(const std::vector<uint8_t>& img, void** d_out, std::vector<void*>* allocs) {
   B2R_CUDA_OK(cudaMalloc(d_out, img.size()));
   allocs->push_back(*d_out);
   B2R_CUDA_OK(cudaMemcpy(*d_out, img.data(), img.size(), cudaMemcpyHostToDevice));
   return B200ROMP_OK;
+}
+
+int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, void** d_out, std::vector<void*>* allocs, int rowb, int eb) {
+  return tc_upload_image(tc_pack_image(w_oihw, cin, cout, taps, nt, rowb, eb), d_out, allocs);
 }
 
 std::string TcConvPlan::describe() const {

@@ -54,7 +54,7 @@ int tc_stem_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t str
 // fused BasicBlock engine (conv_block_tc.cu): y = relu(conv2(relu(conv1(x) + b1)) + b2 + x), 3x3 stride 1, 64 -> 64 -> 64
 // bf16 NHWC.  `p` describes the block as one op: input and residual x (the same channel slice), output y, bias b2; when
 // plan->fold the weights are already the pixel-pair folded ones and `p` the pixel-pair view.
-bool tc_block_supported(const ConvParams& p);
+bool tc_block_supported(const ConvParams& p, bool fold);
 int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
                      TcConvPlan* plan, std::vector<void*>* allocs);
 int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream);

@@ -484,7 +484,7 @@ static void fuse_basic_blocks(b200romp_net* net) {
         f.tc.fold = C == 32;
         ConvParams p;
         fill_params(net, f, 1, true, &p);
-        if (tc_block_supported(p)) {
+        if (tc_block_supported(p, f.tc.fold)) {
           f.mid = t;
           f.lane = a.lane;
           f.w_host = std::move(a.w_host);

@@ -371,7 +371,10 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 PFN_encodeTiled tc_get_encode();
-// bf16 / TF32 weight slab in shared-memory-image order [ntile][tap][chunk][NT rows x ROWB] with the TMA / wgmma XOR swizzle
+// bf16 / TF32 weight slab in shared-memory-image order [ntile][tap][chunk][NT rows x ROWB] with the TMA / wgmma XOR swizzle:
+// tc_pack_image builds it on the host, tc_upload_image copies an image to a new device allocation, tc_pack_weights does both
+std::vector<uint8_t> tc_pack_image(const float* w_oihw, int cin, int cout, int taps, int nt, int rowb, int eb);
+int tc_upload_image(const std::vector<uint8_t>& img, void** d_out, std::vector<void*>* allocs);
 int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, void** d_out, std::vector<void*>* allocs, int rowb, int eb);
 float tc_round_tf32_host(float w);   // fp32 -> TF32, ties away from zero (cvt.rna.tf32.f32)
 
