@@ -300,14 +300,18 @@ int b200romp_preprocess_bgr_batch(const unsigned char* const* imgs_bgr, const in
  * filter state of every track lives in device memory inside the handle.  slot[i] (device int32) = state slot of person i
  * (0 <= slot < max_tracks; a slot whose state was reset initialises on its next sample) or -1 = leave person i untouched.
  * thetas [n,72], betas [n,betas_stride] (first n_betas smoothed), cam [n,3] are updated IN PLACE; the person count is
- * min(n, *d_count) when d_count != NULL.  The track association (norfair in the reference) is the caller's. */
+ * min(n, *d_count) when d_count != NULL.  The track association (norfair in the reference) is the caller's.
+ * tracked selects the recurrence: 0 = --show_largest (main.py:132-135, every filter differentiates against its previous
+ * RAW sample); != 0 = the tracked mode (main.py:148-154), where the reference smooths views of the output rows and writes
+ * the results back into them, so the body-pose, betas and cam filters differentiate against their previous SMOOTHED
+ * value (LowPassFilter keeps the tensor, utils.py:213); the global-rotation filter sees a fresh matrix in both modes. */
 typedef struct b200romp_tracks b200romp_tracks;
 b200romp_tracks* b200romp_tracks_create(int device, int max_tracks);
 void b200romp_tracks_destroy(b200romp_tracks* tracks);
 /* forget the state of one slot (slot >= 0) or of all slots (slot = -1) */
 int b200romp_tracks_reset(b200romp_tracks* tracks, int slot, b200romp_stream stream);
 int b200romp_one_euro_smooth(b200romp_tracks* tracks, const int* slot, int n, const int* d_count, float* thetas, float* betas,
-                             int betas_stride, int n_betas, float* cam, float smooth_coeff, float freq, b200romp_stream stream);
+                             int betas_stride, int n_betas, float* cam, float smooth_coeff, float freq, int tracked, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
  * BEV's video mode (-t/--temporal_optimize, simple_romp/bev/main.py:109-121,165-169,260-287): the reference's 3-D-centre

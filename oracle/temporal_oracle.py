@@ -4,7 +4,8 @@ numpy (fp32) restatement of the reference's One-Euro smoothing: LowPassFilter (s
 OneEuroFilter (:217-246), create_OneEuroFilter (:258-259), smooth_results (:262-270), smooth_global_rot_matrix (:188-192)
 with utils.batch_rodrigues / quat2mat (:493-533) and rotation_matrix_to_angle_axis (:535-552, via the quaternion code
 :554-682 restated in oracle/romp_oracle.py).  Pinned by tests/test_oracle_golden.py::test_one_euro against
-tests/golden/one_euro.npz (outputs of the reference's own functions)."""
+tests/golden/one_euro.npz (outputs of the reference's own functions; the --show_largest recurrence) and
+::test_one_euro_tracked against tests/golden/one_euro_tracked.npz (the tracked recurrence, see smooth_tracked)."""
 import numpy as np
 import torch
 
@@ -62,3 +63,14 @@ def smooth(filters, thetas, betas, cam):
     g = R.rotmat_to_aa(torch.from_numpy(Rm.reshape(1, 3, 3))).numpy().reshape(3)
     pose = filters["smpl_thetas"].process(thetas[3:])
     return np.concatenate([g, pose]).astype(F), filters["smpl_betas"].process(betas), filters["cam"].process(cam)
+
+
+def smooth_tracked(filters, thetas, betas, cam):
+    """One person of the tracked mode (romp/main.py:152-154, bev/main.py:283-285): thetas [72], betas, cam [3] are float32
+    row VIEWS of the frame's outputs and receive the smoothed values in place.  OneEuro.process keeps the view it was
+    given as prev_raw (np.asarray does not copy), as LowPassFilter keeps the tensor (utils.py:213), so the write-back
+    turns prev_raw of body pose, betas and cam into the smoothed value and the next dx is taken against it; the
+    global-rotation filter is fed a fresh matrix and keeps the raw one."""
+    for v in (thetas, betas, cam):
+        assert isinstance(v, np.ndarray) and v.dtype == F and v.base is not None, "smooth_tracked needs float32 row views"
+    thetas[:], betas[:], cam[:] = smooth(filters, thetas, betas, cam)

@@ -162,7 +162,7 @@ def load():
     _sig(lib.b200romp_tracks_create, vp, i32, i32)
     _sig(lib.b200romp_tracks_destroy, None, vp)
     _sig(lib.b200romp_tracks_reset, i32, vp, i32, vp)
-    _sig(lib.b200romp_one_euro_smooth, i32, vp, vp, i32, vp, vp, vp, i32, i32, vp, f32, f32, vp)
+    _sig(lib.b200romp_one_euro_smooth, i32, vp, vp, i32, vp, vp, vp, i32, i32, vp, f32, f32, i32, vp)
     _sig(lib.b200romp_bev_tracker_create, vp, i32, i32, i32)
     _sig(lib.b200romp_bev_tracker_destroy, None, vp)
     _sig(lib.b200romp_bev_tracker_reset, i32, vp, i32, vp)

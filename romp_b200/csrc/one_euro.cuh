@@ -32,7 +32,11 @@ __device__ __forceinline__ void oe_rodrigues(const float* a, float* R) {
 
 // OneEuroFilter.process (:232-246) of one scalar x with the filter state at raw / px / pdx; seen == false: the first
 // sample (dx = 0.0, s = value).  Returns the filtered value.
-__device__ __forceinline__ float oe_step(float x, float mincut, float freq, bool seen, float* raw, float* px, float* pdx) {
+// aliased: the tracked mode of the reference (romp/main.py:152-154, bev/main.py:283-285) hands smooth_results views of
+// the output row and then writes the smoothed values into that row; LowPassFilter keeps prev_raw_value = value without
+// a copy (:213), so the next dx is taken against the SMOOTHED value.  This holds for pose, betas and cam; the rotation
+// matrix is a fresh tensor, and --show_largest rebinds the outputs instead (romp/main.py:133-135), so both keep the raw.
+__device__ __forceinline__ float oe_step(float x, float mincut, float freq, bool seen, bool aliased, float* raw, float* px, float* pdx) {
   float y = x;
   if (seen) {
     const float dx = (x - *raw) * freq;                                              // :233-234
@@ -45,7 +49,7 @@ __device__ __forceinline__ float oe_step(float x, float mincut, float freq, bool
   } else {
     *pdx = 0.0f;
   }
-  *raw = x;
+  *raw = aliased ? y : x;
   *px = y;
   return y;
 }

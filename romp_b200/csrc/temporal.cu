@@ -6,6 +6,8 @@
 // beta 0.7), create_OneEuroFilter :258-259 (mincutoff: thetas = global_rot = smooth_coeff, cam 1.6, betas 0.6),
 // smooth_results :262-270, smooth_global_rot_matrix :188-192 (axis-angle -> matrix via the quaternion form of
 // utils.batch_rodrigues :493-533, filter the 9 entries, rotation_matrix_to_angle_axis :535-552 of the filtered matrix).
+// tracked != 0 is the recurrence of the tracked mode (main.py:148-154: smooth_results on views of the output rows, the
+// smoothed values written back into them), tracked == 0 that of --show_largest (:132-135); see oe_step.
 // The track association itself (norfair in the reference, a third-party tracker that is not part of the repository) is
 // host logic in romp_b200/temporal.py; this file only needs the slot index of every person.
 #include "common.cuh"
@@ -24,7 +26,7 @@ struct OeState {
 // block = one person, thread = one filtered scalar
 __global__ void __launch_bounds__(128) one_euro_kernel(OeState st, const int* __restrict__ slot, int n_host, const int* __restrict__ d_count,
                                                        float* __restrict__ thetas, float* __restrict__ betas, int betas_stride, int n_betas,
-                                                       float* __restrict__ cam, float smooth_coeff, float freq) {
+                                                       float* __restrict__ cam, float smooth_coeff, float freq, int tracked) {
   const int i = blockIdx.x;
   const int N = d_count ? min(n_host, *d_count) : n_host;
   if (i >= N) return;
@@ -44,7 +46,7 @@ __global__ void __launch_bounds__(128) one_euro_kernel(OeState st, const int* __
   float y = x;
   if (active) {
     const size_t o = (size_t)sl * kOeCh + t;
-    y = oe_step(x, mincut, freq, st.seen[sl] != 0, &st.prev_raw[o], &st.prev_x[o], &st.prev_dx[o]);
+    y = oe_step(x, mincut, freq, st.seen[sl] != 0, tracked && t >= kOePose, &st.prev_raw[o], &st.prev_x[o], &st.prev_dx[o]);
   }
   if (t < kOePose) s_R[t] = y;
   else if (t < kOeBeta) thetas[(size_t)i * 72 + 3 + (t - kOePose)] = y;
@@ -104,10 +106,10 @@ int b200romp_tracks_reset(b200romp_tracks* t, int slot, b200romp_stream stream) 
 }
 
 int b200romp_one_euro_smooth(b200romp_tracks* t, const int* slot, int n, const int* d_count, float* thetas, float* betas,
-                             int betas_stride, int n_betas, float* cam, float smooth_coeff, float freq, b200romp_stream stream) {
+                             int betas_stride, int n_betas, float* cam, float smooth_coeff, float freq, int tracked, b200romp_stream stream) {
   B2R_REQUIRE(t && slot && thetas && betas && cam && n > 0 && n_betas > 0 && n_betas <= 16 && betas_stride >= n_betas, "one_euro_smooth: bad arguments");
   B2R_CUDA_OK(cudaSetDevice(t->device));
-  one_euro_kernel<<<n, 128, 0, (cudaStream_t)stream>>>(t->st, slot, n, d_count, thetas, betas, betas_stride, n_betas, cam, smooth_coeff, freq);
+  one_euro_kernel<<<n, 128, 0, (cudaStream_t)stream>>>(t->st, slot, n, d_count, thetas, betas, betas_stride, n_betas, cam, smooth_coeff, freq, tracked);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
 }

@@ -388,11 +388,8 @@ __global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn 
       else { x = in.cam[src * 3 + (c - kOeCam)]; mincut = 1.6f; }
       if (!active) continue;
       const size_t o = (size_t)slot * kOeCh + c;
-      const float y = oe_step(x, mincut, 30.f, seen, &g.oe_raw[o], &g.oe_x[o], &g.oe_dx[o]);
-      // bev/main.py:283-285 passes views of the output row to smooth_results and then writes the smoothed values into
-      // that row, so the filters' prev_raw_value of pose, betas and cam becomes the smoothed value (the rotation
-      // matrix is a fresh tensor; --show_largest rebinds the outputs instead, :264-266)
-      if (!in.show_largest && c >= kOePose) g.oe_raw[o] = y;
+      // tracked mode: pose, betas and cam differentiate against their previous smoothed value (oe_step, aliased)
+      const float y = oe_step(x, mincut, 30.f, seen, !in.show_largest && c >= kOePose, &g.oe_raw[o], &g.oe_x[o], &g.oe_dx[o]);
       if (c < kOePose) s.R[r][c] = y;
       else if (c < kOeBeta) out.thetas[dst * 72 + 3 + (c - kOePose)] = y;
       else if (c < kOeCam) out.betas[dst * 11 + (c - kOeBeta)] = y;

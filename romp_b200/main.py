@@ -603,7 +603,8 @@ class ROMP(torch.nn.Module):
         with torch.cuda.stream(self.stream):
             self._slot_dev[:n].copy_(self._slot_host[:n], non_blocking=True)
             _lib.check(lib.b200romp_one_euro_smooth(self._tracks, _ptr(self._slot_dev), n, None, _ptr(b["thetas"]), _ptr(b["betas"]),
-                                                    10, 10, _ptr(b["cam"]), float(self.settings.smooth_coeff), 30.0, sp), "one_euro")
+                                                    10, 10, _ptr(b["cam"]), float(self.settings.smooth_coeff), 30.0,
+                                                    int(not self.temporal.show_largest), sp), "one_euro")
             if self.temporal.show_largest:                 # only the largest person goes on (main.py:129-134)
                 k = int(np.argmax(cams[:, 0]))
                 for key in ("thetas", "betas", "cam"):

@@ -11,7 +11,11 @@ person uses.
   tracked object (utils.py:275-280).  ``norfair`` is a third-party package that is neither vendored in the reference nor
   installed here (the reference pip-installs it on demand, main.py:120-125), so its Kalman-filter tracker is NOT
   restated: ``NearestCenterTracker`` below is a plain nearest-neighbour association with the same distance threshold -
-  "parity unpinned" for the ids; the filters themselves are pinned to the reference (tests/golden/one_euro.npz).
+  "parity unpinned" for the ids, which remain so; the filter recurrence is the reference's in both modes: --show_largest
+  differentiates against the previous raw sample (tests/golden/one_euro.npz), the tracked mode - where the reference
+  smooths views of the output rows and writes the results back into them (main.py:152-154) - against the previous
+  smoothed value of body pose, betas and cam (tests/golden/one_euro_tracked.npz); ``b200romp_one_euro_smooth`` takes
+  the mode as its ``tracked`` argument.
 """
 from __future__ import annotations
 

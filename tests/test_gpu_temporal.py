@@ -1,6 +1,8 @@
 """Row f4 on the GPU: the One-Euro smoothing stage (csrc/temporal.cu) through the C ABI against the REFERENCE's own
 smooth_results outputs (tests/golden/one_euro.npz), with interleaved slots and a slot reset; and ROMP.forward with
---temporal_optimize (both the --show_largest and the tracked mode) on a short synthetic sequence."""
+--temporal_optimize (both the --show_largest and the tracked mode) on a short synthetic sequence; the tracked mode against
+the oracle's tracked recurrence (oracle/temporal_oracle.py::smooth_tracked) fed with the plain model's outputs and the
+ids the run returned.  The kernel's two recurrences against float64: tests/test_gpu_romp_post_fp64.py."""
 import ctypes as C
 import os
 
@@ -30,7 +32,7 @@ def test_one_euro_kernel_matches_reference_sequences():
             be = torch.from_numpy(z["betas"][t]).cuda().contiguous()
             ca = torch.from_numpy(z["cam"][t]).cuda().contiguous()
             _lib.check(lib.b200romp_one_euro_smooth(h, C.c_void_p(slots.data_ptr()), P, None, C.c_void_p(th.data_ptr()),
-                                                    C.c_void_p(be.data_ptr()), 10, 10, C.c_void_p(ca.data_ptr()), 3.0, 30.0, st))
+                                                    C.c_void_p(be.data_ptr()), 10, 10, C.c_void_p(ca.data_ptr()), 3.0, 30.0, 0, st))
             torch.cuda.synchronize()
             err = max(err, np.abs(th.cpu().numpy() - z["out_thetas"][t]).max(), np.abs(be.cpu().numpy() - z["out_betas"][t]).max(),
                       np.abs(ca.cpu().numpy() - z["out_cam"][t]).max())
@@ -42,6 +44,7 @@ def test_one_euro_kernel_matches_reference_sequences():
 @pytest.mark.parametrize("largest", [False, True])
 def test_forward_with_temporal_optimize(largest):
     from oracle import romp_oracle as O
+    from oracle import temporal_oracle as T
     sd, pack = synth.romp_state_dict(0), synth.smpl_pack(0)
     rs = np.random.RandomState(7)
     base = rs.randint(0, 256, (512, 512, 3)).astype(np.uint8)
@@ -50,8 +53,8 @@ def test_forward_with_temporal_optimize(largest):
     flags = ["--precision", "fp32", "--max_batch", "1", "-t"] + (["--show_largest"] if largest else [])
     m = ROMP(romp_settings(flags), state_dict=sd2, smpl_pack=pack)
     plain = ROMP(romp_settings(["--precision", "fp32", "--max_batch", "1"]), state_dict=sd2, smpl_pack=pack)
-    outs = []
-    for t in range(3):
+    outs, filters = [], {}
+    for t in range(6):
         img = np.clip(base.astype(np.int32) + rs.randint(-6, 7, base.shape), 0, 255).astype(np.uint8)   # small frame-to-frame change
         o, p = m(img), plain(img)
         assert o is not None and p is not None
@@ -65,6 +68,13 @@ def test_forward_with_temporal_optimize(largest):
             k = int(np.argmax(p["cam"][:, 0])) if largest else slice(None)
             assert np.abs(o["cam"] - p["cam"][k]).max() < 1e-6 and np.abs(o["smpl_thetas"][..., 3:] - p["smpl_thetas"][k][..., 3:]).max() < 1e-6
             assert np.abs(o["smpl_thetas"][..., :3] - p["smpl_thetas"][k][..., :3]).max() < 1e-4
+        if not largest:  # every frame equals the reference's tracked recurrence on the unsmoothed outputs (departs at frame 2 otherwise)
+            th, be, ca = p["smpl_thetas"].copy(), p["smpl_betas"].copy(), p["cam"].copy()
+            first = {int(tid): r for r, tid in reversed(list(enumerate(o["track_ids"])))}
+            for tid, r in first.items():     # a second detection on one track in a frame is left unsmoothed (temporal.py)
+                T.smooth_tracked(filters.setdefault(tid, T.make_filters(3.0)), th[r], be[r], ca[r])
+            assert np.abs(o["smpl_thetas"][:, 3:] - th[:, 3:]).max() < 3e-5, t
+            assert np.abs(o["smpl_betas"] - be).max() < 3e-5 and np.abs(o["cam"] - ca).max() < 3e-5, t
         # SMPL ran on the smoothed parameters
         v, j = O.smpl_forward(pack, o["smpl_betas"], o["smpl_thetas"])
         assert np.abs(o["verts"] - v.numpy()).max() < 1e-4

@@ -137,3 +137,46 @@ def test_one_euro(golden_dir):
             a, b, c = T.smooth(filters[p], z["thetas"][t, p], z["betas"][t, p], z["cam"][t, p])
             err = max(err, np.abs(a - z["out_thetas"][t, p]).max(), np.abs(b - z["out_betas"][t, p]).max(), np.abs(c - z["out_cam"][t, p]).max())
     assert err < 2e-5, err
+
+
+def run_tracked_fixture(z, step):
+    """Drive step(filters, thetas_row, betas_row, cam_row) over the tracked fixture the way romp/main.py:148-154 does;
+    -> max |err| per frame [T]."""
+    from oracle import temporal_oracle as T
+    filters, errs = {}, []
+    for t in range(len(z["n"])):
+        n = int(z["n"][t])
+        th, be, ca = z["thetas"][t, :n].copy(), z["betas"][t, :n].copy(), z["cam"][t, :n].copy()
+        for r, tid in enumerate(z["ids"][t, :n].tolist()):
+            step(filters.setdefault(tid, T.make_filters(3.0)), th[r], be[r], ca[r])
+        errs.append(max(np.abs(th - z["out_thetas"][t, :n]).max(), np.abs(be - z["out_betas"][t, :n]).max(),
+                        np.abs(ca - z["out_cam"][t, :n]).max()))
+    return np.array(errs)
+
+
+def test_one_euro_tracked(golden_dir):
+    """The tracked recurrence (smooth_results on row views, results written back: the pose, betas and cam filters see
+    their previous smoothed value as prev_raw) against the reference driven as romp/main.py:148-154 drives it.  The
+    non-aliased recurrence of --show_largest must NOT reproduce this fixture (it departs at every track's third sample),
+    nor the aliased one the --show_largest fixture."""
+    from oracle import temporal_oracle as T
+    z = g(golden_dir, "one_euro_tracked.npz")
+    assert len(z["n"]) >= 40 and z["n"].max() == 6 and z["n"].min() < 6
+    err = run_tracked_fixture(z, T.smooth_tracked)
+    assert err.max() < 2e-5, err
+
+    def plain(f, th, be, ca):
+        th[:], be[:], ca[:] = T.smooth(f, th.copy(), be.copy(), ca.copy())
+    err = run_tracked_fixture(z, plain)
+    assert err[:2].max() < 2e-5 and err[2] > 1e-3 and (err[2:] > 3e-5).all(), err
+
+    z = g(golden_dir, "one_euro.npz")
+    Tn, P = z["thetas"].shape[:2]
+    filters = [T.make_filters(3.0) for _ in range(P)]
+    errs = []
+    for t in range(Tn):
+        th, be, ca = z["thetas"][t].copy(), z["betas"][t].copy(), z["cam"][t].copy()
+        for p in range(P):
+            T.smooth_tracked(filters[p], th[p], be[p], ca[p])
+        errs.append(max(np.abs(th - z["out_thetas"][t]).max(), np.abs(be - z["out_betas"][t]).max(), np.abs(ca - z["out_cam"][t]).max()))
+    assert max(errs[:2]) < 2e-5 and min(errs[2:]) > 3e-5, errs
