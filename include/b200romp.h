@@ -234,18 +234,20 @@ int b200romp_bev_regress(b200romp_bev* bev, const float* maps_fv, const void* bv
 /* After SMPL-A (into verts/joints) and SMIL (into verts_smil/joints_smil, may be NULL): merge babies (betas[:,10] > 0.8,
  * bev/post_parser.py:255-278), perspective projection to original-image pixels (:68-107,129-152), then per frame
  * suppressing_redundant_prediction_via_projection and remove_outlier (:167-222).  keep[cap] flags, sel[cap] = indices of
- * the survivors in order, *d_count_out = their number. */
+ * the survivors in order, *d_count_out = their number.  Suppression threshold in pixels: (float)(nms_thresh *
+ * max(img_max_side, 3) / 640) formed in double, what torch compares with for an image of shape (h, w, 3) with
+ * img_max_side = max(h, w) (bev/main.py:179). */
 int b200romp_bev_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                       const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
-                      const int* d_count, const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side,
+                      const int* d_count, const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side,
                       float* pj2d_org, int* keep, int* sel, int* d_count_out, b200romp_stream stream);
 /* b200romp_bev_post for a batch of frames of different sizes: the host offsets6 / img_max_side are replaced by the DEVICE
  * fp32 [batch,6] pad_table ([top,bottom,left,right,h,w] per frame).  Each frame projects with its own size, left and top
- * (bev/post_parser.py:129-152) and suppresses with its own threshold nms_thresh * max(h,w) / 640 (:148-149,186-187) - what
+ * (bev/post_parser.py:129-152) and suppresses with its own threshold (float)(nms_thresh * max(h,w,3) / 640) (:148-149,186-187) - what
  * BEV.process_normal_image (bev/main.py:158-181) does for one image. */
 int b200romp_bev_post_frames(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                              const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
-                             const int* d_count, const float* pad_table, float nms_thresh, float rel_scale_thresh, float* pj2d_org,
+                             const int* d_count, const float* pad_table, double nms_thresh, float rel_scale_thresh, float* pj2d_org,
                              int* keep, int* sel, int* d_count_out, b200romp_stream stream);
 /* Long-image (crowd) mode, per-crop stage (bev/main.py:196-249, bev/split2process.py:41-58) for one chunk of crop frames
  * (batch frames = crops crop0 .. crop0+batch-1 of the image, rows grouped by frame like bev_parse3d leaves them).  After
@@ -266,12 +268,12 @@ int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const fl
                            float* acc_params_pred, float* acc_conf, float* acc_cam, b200romp_stream stream);
 /* Long-image mode, merged stage (bev/main.py:253-256) over the *d_count accumulated persons of one image (any number up
  * to capacity, not bounded by 64): cam_trans from the full-image cam, projection with the full image's pad info
- * offsets6 (HOST, [top,bottom,left,right,h,w]), conf-based suppression with nms_thresh * img_max_side / 640 (every pair below
+ * offsets6 (HOST, [top,bottom,left,right,h,w]), conf-based suppression with (float)(nms_thresh * max(img_max_side,3) / 640) (every pair below
  * it at once), remove_outlier(scale_thresh=0.5).  removed [cap] flags; sel [cap] = survivors in order, *d_count_out their
  * number.  workspace: b200romp_bev_long_merge_workspace_bytes(capacity) bytes of device memory. */
 long long b200romp_bev_long_merge_workspace_bytes(int capacity);
 int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
-                            const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
+                            const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
                             float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream);
 /* dst[i] = src[sel[i]] for i < *d_count; rows of row_bytes (multiple of 4) bytes. */
 int b200romp_gather_rows(const void* src, int row_bytes, const int* sel, const int* d_count, int capacity, void* dst,

@@ -116,7 +116,7 @@ def load():
             f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
             "(romp_b200 has no fallback path without its CUDA library)")
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
-    vp, i32, f32, i64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong
+    vp, i32, f32, f64, i64 = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_longlong
     fp, ip, lp = C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_longlong)
     _sig(lib.b200romp_version, i32)
     _sig(lib.b200romp_last_error, C.c_char_p)
@@ -153,11 +153,11 @@ def load():
     _sig(lib.b200romp_bev_parse_workspace_bytes, i64, i32)
     _sig(lib.b200romp_bev_parse3d, i32, vp, i32, f32, i32, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_regress, i32, vp, vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
-    _sig(lib.b200romp_bev_post, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp)
-    _sig(lib.b200romp_bev_post_frames, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, f32, f32, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_bev_post, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, fp, f64, f32, f32, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_bev_post_frames, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, f64, f32, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_crop_post, i32, *([vp] * 11), i32, i32, vp, vp, i32, f32, vp, vp, vp, vp, i32, *([vp] * 9), vp)
     _sig(lib.b200romp_bev_long_merge_workspace_bytes, i64, i32)
-    _sig(lib.b200romp_bev_long_merge, i32, vp, vp, vp, i32, vp, fp, f32, f32, f32, vp, vp, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_bev_long_merge, i32, vp, vp, vp, i32, vp, fp, f64, f32, f32, vp, vp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_gather_rows, i32, vp, i32, vp, vp, i32, vp, vp)
     _sig(lib.b200romp_tracks_create, vp, i32, i32)
     _sig(lib.b200romp_tracks_destroy, None, vp)

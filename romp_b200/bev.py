@@ -607,7 +607,8 @@ class BEV(torch.nn.Module):
                 raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
             return self.process_long_image(image)
         inp, pad = img_preprocess(image)
-        out = self.forward_batch(torch.from_numpy(inp), offsets=pad, img_max_side=float(max(image.shape[:2])), signal_IDs=[signal_ID])
+        # the reference suppresses with max(image.shape), channels included (bev/main.py:179)
+        out = self.forward_batch(torch.from_numpy(inp), offsets=pad, img_max_side=float(max(*image.shape[:2], 3)), signal_IDs=[signal_ID])
         if out is None:
             print("No person detected!")                                       # bev/model.py:239
             return None

@@ -468,6 +468,13 @@ __global__ void __launch_bounds__(128) bev_project_kernel(const float* __restric
   pj2d_org[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f - top;
 }
 
+// Suppression threshold in pixels, bev/post_parser.py:186-188: thresh * max(img_shape) / 640 in double, where img_shape is
+// the image's (h, w, 3) (bev/main.py:179,255), so the largest side counts as at least 3; torch then compares the fp32
+// normalised distances with that number rounded to fp32.
+__host__ __device__ __forceinline__ float nms_thr_px_of(double nms_thresh, float max_side) {
+  return (float)(nms_thresh * fmax((double)max_side, 3.0) / 640.0);
+}
+
 // [start, start + n) = the rows of frame b (rows are grouped by frame, in frame order); n capped at cap
 __device__ __forceinline__ void frame_rows(const long long* __restrict__ batch_ids, int N, int b, int* s_start, int* s_n, int cap = kMaxP) {
   int s = 0;
@@ -520,15 +527,25 @@ __device__ void postfilter_frame(const float* __restrict__ pj2d_org, const float
   const int nk = *s_nk;
   if (nk >= 3) {
     if (tid < nk) {
+      // mean of the sorted distance row without its first entry (the self-distance, exactly 0, so it adds nothing) and
+      // its last (the row maximum): the row is summed without the first index that attains the maximum, so a far person
+      // does not cancel against the sum the way (sum - min - max) does
       const float* ti = cam_trans + (size_t)(st + s_kept[tid]) * 3;
-      float sum = 0.f, mn = CUDART_INF_F, mx = -CUDART_INF_F;
-      for (int j = 0; j < nk; ++j) {
+      auto dist = [&](int j) {
         const float* tj = cam_trans + (size_t)(st + s_kept[j]) * 3;
         const float dx = ti[0] - tj[0], dy = ti[1] - tj[1], dz = ti[2] - tj[2];
-        const float d = sqrtf(dx * dx + dy * dy + dz * dz);
-        sum += d; mn = fminf(mn, d); mx = fmaxf(mx, d);
+        return sqrtf(dx * dx + dy * dy + dz * dz);
+      };
+      float mx = -CUDART_INF_F;
+      int imx = 0;
+      for (int j = 0; j < nk; ++j) {
+        const float d = dist(j);
+        if (d > mx) { mx = d; imx = j; }
       }
-      s_mean[tid] = (sum - mn - mx) / (float)(nk - 2);       // sorted row without its first and last entry
+      float sum = 0.f;
+      for (int j = 0; j < nk; ++j)
+        if (j != imx) sum += dist(j);
+      s_mean[tid] = sum / (float)(nk - 2);
     }
     __syncthreads();
     if (tid < nk) {
@@ -547,15 +564,13 @@ template <int CAP>
 __global__ void __launch_bounds__(256) bev_postfilter_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
                                                              const float* __restrict__ cam_trans, const long long* __restrict__ batch_ids,
                                                              const int* __restrict__ d_count, float nms_thr_px, float rel_scale_thresh,
-                                                             const float* __restrict__ pad_tab, float nms_thresh, int* __restrict__ keep) {
+                                                             const float* __restrict__ pad_tab, double nms_thresh, int* __restrict__ keep) {
   __shared__ int s_start, s_n;
   __shared__ int s_drop[CAP], s_removed[CAP], s_kept[CAP], s_nk;
   __shared__ float s_mean[CAP];
   const int b = blockIdx.x, tid = threadIdx.x;
-  if (pad_tab) {                       // this frame's own threshold nms_thresh * max(h, w) / 640 (bev/post_parser.py:186-187)
-    const float h = pad_tab[b * 6 + 4], w = pad_tab[b * 6 + 5];
-    nms_thr_px = __fdiv_rn(__fmul_rn(nms_thresh, h > w ? h : w), 640.f);
-  }
+  if (pad_tab)                         // this frame's own threshold (bev/post_parser.py:186-187), see nms_thr_px_of
+    nms_thr_px = nms_thr_px_of(nms_thresh, fmaxf(pad_tab[b * 6 + 4], pad_tab[b * 6 + 5]));
   if (tid == 0) frame_rows(batch_ids, *d_count, b, &s_start, &s_n, CAP);
   if (tid < CAP) s_drop[tid] = 0;
   __syncthreads();
@@ -731,33 +746,48 @@ __global__ void __launch_bounds__(1024) bev_long_kept_kernel(const int* __restri
   if (threadIdx.x == 0) *ws_nk = k;
 }
 
-// remove_outlier, mean of each survivor's sorted distance row without its first and last entry: one CTA per survivor
+// remove_outlier, mean of each survivor's sorted distance row without its first and last entry: one CTA per survivor.
+// The first entry is the self-distance (exactly 0), the last the row maximum; the row is summed without the first index
+// that attains the maximum (a (max, smallest index) reduction, then a second pass), so a far person does not cancel
+// against the sum the way (sum - min - max) does.
 __global__ void __launch_bounds__(128) bev_long_meandist_kernel(const float* __restrict__ cam_trans, const int* __restrict__ ws_sel,
                                                                 const int* __restrict__ ws_nk, float* __restrict__ ws_mean) {
   const int nk = *ws_nk, r = blockIdx.x;
   if (nk < 3 || r >= nk) return;
   const float* ti = cam_trans + (size_t)ws_sel[r] * 3;
-  float sum = 0.f, mn = CUDART_INF_F, mx = -CUDART_INF_F;
-  for (int k = threadIdx.x; k < nk; k += 128) {
+  auto dist = [&](int k) {
     const float* tj = cam_trans + (size_t)ws_sel[k] * 3;
     const float dx = ti[0] - tj[0], dy = ti[1] - tj[1], dz = ti[2] - tj[2];
-    const float d = sqrtf(dx * dx + dy * dy + dz * dz);
-    sum += d; mn = fminf(mn, d); mx = fmaxf(mx, d);
+    return sqrtf(dx * dx + dy * dy + dz * dz);
+  };
+  float mx = -CUDART_INF_F;
+  int imx = nk;
+  for (int k = threadIdx.x; k < nk; k += 128) {
+    const float d = dist(k);
+    if (d > mx) { mx = d; imx = k; }
   }
-  __shared__ float s_sum[4], s_mn[4], s_mx[4];
+  __shared__ float s_mx[4], s_sum[4];
+  __shared__ int s_imx[4];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
-    sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, imx, o);
+    if (om > mx || (om == mx && oi < imx)) { mx = om; imx = oi; }
   }
-  if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = sum; s_mn[threadIdx.x >> 5] = mn; s_mx[threadIdx.x >> 5] = mx; }
+  if ((threadIdx.x & 31) == 0) { s_mx[threadIdx.x >> 5] = mx; s_imx[threadIdx.x >> 5] = imx; }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    const float s = s_sum[0] + s_sum[1] + s_sum[2] + s_sum[3];
-    const float lo = fminf(fminf(s_mn[0], s_mn[1]), fminf(s_mn[2], s_mn[3])), hi = fmaxf(fmaxf(s_mx[0], s_mx[1]), fmaxf(s_mx[2], s_mx[3]));
-    ws_mean[r] = (s - lo - hi) / (float)(nk - 2);
-  }
+  mx = s_mx[0]; imx = s_imx[0];
+#pragma unroll
+  for (int w = 1; w < 4; ++w)
+    if (s_mx[w] > mx || (s_mx[w] == mx && s_imx[w] < imx)) { mx = s_mx[w]; imx = s_imx[w]; }
+  float sum = 0.f;
+  for (int k = threadIdx.x; k < nk; k += 128)
+    if (k != imx) sum += dist(k);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if ((threadIdx.x & 31) == 0) s_sum[threadIdx.x >> 5] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) ws_mean[r] = (s_sum[0] + s_sum[1] + s_sum[2] + s_sum[3]) / (float)(nk - 2);
 }
 
 // relative scale of every survivor against the others, outliers (and cam[:,0] < scale_thresh) removed, final compaction
@@ -945,7 +975,7 @@ int b200romp_bev_regress(b200romp_bev* h, const float* maps_fv, const void* bv_o
 
 static int bev_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints, const float* cam,
                     const float* cam_trans, const long long* batch_ids, int batch, int capacity, const int* d_count, const float* offsets6,
-                    const float* pad_table, float nms_thresh, float rel_scale_thresh, float img_max_side, float* pj2d_org, int* keep,
+                    const float* pad_table, double nms_thresh, float rel_scale_thresh, float img_max_side, float* pj2d_org, int* keep,
                     int* sel, int* d_count_out, cudaStream_t stream) {
   if (verts_smil && joints_smil)
     bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
@@ -956,13 +986,13 @@ static int bev_post(const float* betas, const float* verts_smil, const float* jo
   }
   bev_project_kernel<<<capacity, 128, 0, stream>>>(joints, cam_trans, d_count, size, left, top, pad_table, batch_ids, pj2d_org);
   B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
+  const float thr_px = nms_thr_px_of(nms_thresh, img_max_side);      // not used with a pad table
   if (capacity > batch * kMaxP)
-    bev_postfilter_kernel<2 * kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count,
-                                                                nms_thresh * img_max_side / 640.f, rel_scale_thresh, pad_table,
-                                                                nms_thresh, keep);
+    bev_postfilter_kernel<2 * kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, thr_px, rel_scale_thresh,
+                                                                pad_table, nms_thresh, keep);
   else
-    bev_postfilter_kernel<kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, nms_thresh * img_max_side / 640.f,
-                                                            rel_scale_thresh, pad_table, nms_thresh, keep);
+    bev_postfilter_kernel<kMaxP><<<batch, 256, 0, stream>>>(pj2d_org, cam, cam_trans, batch_ids, d_count, thr_px, rel_scale_thresh,
+                                                            pad_table, nms_thresh, keep);
   bev_compact_kernel<<<1, 32, 0, stream>>>(keep, d_count, sel, d_count_out);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
@@ -970,7 +1000,7 @@ static int bev_post(const float* betas, const float* verts_smil, const float* jo
 
 int b200romp_bev_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                       const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
-                      const int* d_count, const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side,
+                      const int* d_count, const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side,
                       float* pj2d_org, int* keep, int* sel, int* d_count_out, b200romp_stream stream_) {
   B2R_REQUIRE(betas && verts && joints && cam && cam_trans && batch_ids && d_count && offsets6 && pj2d_org && keep && sel &&
                   d_count_out && batch > 0 && capacity > 0, "bev_post: bad arguments");
@@ -980,7 +1010,7 @@ int b200romp_bev_post(const float* betas, const float* verts_smil, const float* 
 
 int b200romp_bev_post_frames(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                              const float* cam, const float* cam_trans, const long long* batch_ids, int batch, int capacity,
-                             const int* d_count, const float* pad_table, float nms_thresh, float rel_scale_thresh, float* pj2d_org,
+                             const int* d_count, const float* pad_table, double nms_thresh, float rel_scale_thresh, float* pj2d_org,
                              int* keep, int* sel, int* d_count_out, b200romp_stream stream_) {
   B2R_REQUIRE(betas && verts && joints && cam && cam_trans && batch_ids && d_count && pad_table && pj2d_org && keep && sel &&
                   d_count_out && batch > 0 && capacity > 0, "bev_post_frames: bad arguments");
@@ -1018,7 +1048,7 @@ int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const fl
 long long b200romp_bev_long_merge_workspace_bytes(int capacity) { return (long long)capacity * 8 + 16; }
 
 int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
-                            const float* offsets6, float nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
+                            const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
                             float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream_) {
   B2R_REQUIRE(cam && joints && conf && d_count && offsets6 && cam_trans && pj2d_org && removed && workspace && sel && d_count_out &&
                   capacity > 0 && img_max_side > 0.f, "bev_long_merge: bad arguments");
@@ -1029,8 +1059,8 @@ int b200romp_bev_long_merge(const float* cam, const float* joints, const float* 
   const float top = offsets6[0], left = offsets6[2], hh = offsets6[4], ww = offsets6[5];
   bev_long_project_kernel<<<capacity, 128, 0, stream>>>(cam, joints, d_count, hh > ww ? hh : ww, left, top, cam_trans, pj2d_org, removed);
   const unsigned tiles = (unsigned)((capacity + kPT - 1) / kPT);
-  bev_long_pairs_kernel<<<dim3(tiles, tiles), 256, 0, stream>>>(pj2d_org, cam, conf, d_count,
-                                                                (float)((double)nms_thresh * img_max_side / 640.0), removed);
+  bev_long_pairs_kernel<<<dim3(tiles, tiles), 256, 0, stream>>>(pj2d_org, cam, conf, d_count, nms_thr_px_of(nms_thresh, img_max_side),
+                                                                removed);
   bev_long_kept_kernel<<<1, 1024, 0, stream>>>(removed, d_count, ws_sel, ws_nk);
   bev_long_meandist_kernel<<<capacity, 128, 0, stream>>>(cam_trans, ws_sel, ws_nk, ws_mean);
   bev_long_outlier_kernel<<<1, 1024, 0, stream>>>(cam, ws_sel, ws_nk, ws_mean, rel_scale_thresh, 0.5f, sel, d_count_out);
