@@ -5,12 +5,15 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <vector>
 
 #include "../../include/b200romp.h"
 
 namespace b200romp {
 
 void set_error(const char* fmt, ...);
+// copies `bytes` of host memory to a new device allocation, recorded in `allocs`; nullptr (error set) on failure
+void* upload(const void* host, size_t bytes, std::vector<void*>* allocs);
 // -1 = default; 0 = launch the next tensor-core convs without the programmatic-dependent-launch attribute (net.cu: ops that wait
 // for another lane inside the captured graph).  Defined in conv_tc.cu.
 extern thread_local int g_tc_pdl_override;

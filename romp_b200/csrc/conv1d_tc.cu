@@ -112,17 +112,12 @@ bool tc_conv1d_supported(const ConvParams& p) {
 }
 
 static int conv1d_encode(const ConvParams& p, TcConvPlan* plan) {
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) { set_error("conv1d_tc: cuTensorMapEncodeTiled is unavailable"); return B200ROMP_ECUDA; }
-  CUtensorMap tm;
   const cuuint64_t gdim[3] = {(cuuint64_t)p.in_C, (cuuint64_t)p.Win, (cuuint64_t)p.B * p.Hin};
   const cuuint64_t gstr[2] = {(cuuint64_t)p.in_C * 2, (cuuint64_t)p.Win * p.in_C * 2};
   const cuuint32_t box[3] = {64, (cuuint32_t)k1dARows, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult cr = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(p.in), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) { set_error("conv1d_tc: cuTensorMapEncodeTiled failed with %d", (int)cr); return B200ROMP_ECUDA; }
-  memcpy(plan->tmap_in, &tm, sizeof(tm));
+  int rc = tc_encode_tiled(&plan->tmap_in, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.in, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                           "conv1d_tc");
+  if (rc) return rc;
   plan->encoded_in = p.in;
   plan->encoded_batch = p.B;
   return B200ROMP_OK;
@@ -135,12 +130,10 @@ static int conv1d_inst(const TcConvPlan& plan, const ConvParams& p, cudaStream_t
     B2R_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     return B200ROMP_OK;
   }
-  CUtensorMap tm;
-  memcpy(&tm, plan.tmap_in, sizeof(tm));
   const int tiles_w = p.Wout / 128, num_tiles = tiles_w * p.Hout * p.B;
   dim3 grid(std::min(plan.grid_x, num_tiles), plan.grid_y);
-  B2R_CUDA_OK(tc_launch(kern, grid, k1dThreads, plan.smem_bytes, stream, tm, p, reinterpret_cast<const uint8_t*>(plan.d_wpack), plan.cin / 64,
-                        tiles_w, num_tiles, plan.stages));
+  B2R_CUDA_OK(tc_launch(kern, grid, k1dThreads, plan.smem_bytes, stream, plan.tmap_in, p, reinterpret_cast<const uint8_t*>(plan.d_wpack),
+                        plan.cin / 64, tiles_w, num_tiles, plan.stages));
   return B200ROMP_OK;
 }
 
@@ -167,9 +160,8 @@ int tc_conv1d_prepare(const ConvParams& p, const float* w_oi3, int sm_count, TcC
             tile[byte / 2] = __float2bfloat16_rn(w);
           }
       }
-  B2R_CUDA_OK(cudaMalloc(&plan->d_wpack, img.size() * sizeof(__nv_bfloat16)));
-  allocs->push_back(plan->d_wpack);
-  B2R_CUDA_OK(cudaMemcpy(plan->d_wpack, img.data(), img.size() * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice));
+  plan->d_wpack = upload(img.data(), img.size() * sizeof(__nv_bfloat16), allocs);
+  if (!plan->d_wpack) return B200ROMP_ECUDA;
   if (!tc_get_encode()) {   // resolved now rather than at the first launch, which may be inside a stream capture
     set_error("conv1d_tc: cuTensorMapEncodeTiled is unavailable");
     return B200ROMP_ECUDA;

@@ -355,16 +355,12 @@ static int block_pack_weights(const float* w_oihw, bool fold, void** d_out, std:
     if (tap % 3 == 1) memcpy(dst, full.data() + (size_t)tap * kTapBytes, kTapBytes);
     else memcpy(dst, half.data() + (size_t)(2 * tap + (tap % 3 == 0 ? 1 : 0)) * kHalfTapBytes, kHalfTapBytes);
   }
-  return tc_upload_image(img, d_out, allocs);
+  *d_out = upload(img.data(), img.size(), allocs);
+  return *d_out ? B200ROMP_OK : B200ROMP_ECUDA;
 }
 
 int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, int sm_count,
                      TcConvPlan* plan, std::vector<void*>* allocs) {
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) {
-    set_error("conv_block_tc: cuTensorMapEncodeTiled is unavailable");
-    return B200ROMP_ECUDA;
-  }
   plan->kind = 60;
   plan->eb = 2;
   plan->cin = plan->cout = plan->nt = 64;
@@ -376,38 +372,23 @@ int tc_block_prepare(const ConvParams& p, const float* w1_oihw, const float* b1,
   if (rc) return rc;
   rc = block_pack_weights(w2_oihw, plan->fold, &plan->d_wpack2, allocs);
   if (rc) return rc;
-  void* db1 = nullptr;
-  B2R_CUDA_OK(cudaMalloc(&db1, 64 * sizeof(float)));
-  allocs->push_back(db1);
-  B2R_CUDA_OK(cudaMemcpy(db1, b1, 64 * sizeof(float), cudaMemcpyHostToDevice));
-  plan->d_bias1 = static_cast<const float*>(db1);
-  // tensor map over the NHWC input slice: dims (C, W, H, N), 20 x (TW + 4) halo box, OOB -> zeros
-  CUtensorMap tm;
-  const cuuint64_t gdim[4] = {64, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
-  const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * 2, (cuuint64_t)p.Win * p.in_C * 2, (cuuint64_t)p.Hin * p.Win * p.in_C * 2};
-  const cuuint32_t box[4] = {64, (cuuint32_t)(plan->fold ? BlkCfg<true>::kHaloW : BlkCfg<false>::kHaloW), kHaloH, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * 2);
-  CUresult cr = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    set_error("conv_block_tc: cuTensorMapEncodeTiled failed with %d", (int)cr);
-    return B200ROMP_ECUDA;
-  }
-  memcpy(plan->tmap_in, &tm, sizeof(tm));
+  plan->d_bias1 = static_cast<const float*>(upload(b1, 64 * sizeof(float), allocs));
+  if (!plan->d_bias1) return B200ROMP_ECUDA;
+  // the 64-channel input slice with a 20 x (TW + 4) halo box
+  rc = tc_encode_nhwc_input(&plan->tmap_in, p, 2, 64, plan->fold ? BlkCfg<true>::kHaloW : BlkCfg<false>::kHaloW, kHaloH,
+                            CU_TENSOR_MAP_SWIZZLE_128B, "conv_block_tc");
+  if (rc) return rc;
   B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BlkCfg<false>::kSmemBytes));
   B2R_CUDA_OK(cudaFuncSetAttribute(conv_block_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BlkCfg<true>::kSmemBytes));
   return B200ROMP_OK;
 }
 
 int tc_block_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) {
-  CUtensorMap tm;
-  memcpy(&tm, plan.tmap_in, sizeof(tm));
   const int tiles_x = p.Wout / (plan.fold ? BlkCfg<true>::kTW : BlkCfg<false>::kTW), tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   const dim3 grid(std::min(plan.grid_x, num_tiles));
   auto kern = plan.fold ? conv_block_tc_kernel<true> : conv_block_tc_kernel<false>;
-  B2R_CUDA_OK(tc_launch(kern, grid, kBlkThreads, plan.smem_bytes, stream, tm, p, reinterpret_cast<const uint8_t*>(plan.d_wpack),
+  B2R_CUDA_OK(tc_launch(kern, grid, kBlkThreads, plan.smem_bytes, stream, plan.tmap_in, p, reinterpret_cast<const uint8_t*>(plan.d_wpack),
                         reinterpret_cast<const uint8_t*>(plan.d_wpack2), plan.d_bias1, tiles_x, tiles_y, num_tiles));
   return B200ROMP_OK;
 }

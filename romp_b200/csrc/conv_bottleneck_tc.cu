@@ -299,22 +299,8 @@ bool tc_bottleneck_supported(const ConvParams& p) {
   return (reinterpret_cast<uintptr_t>(p.in) & 15) == 0;
 }
 
-static int upload_floats(const float* h, int n, const float** d, std::vector<void*>* allocs) {
-  void* dp = nullptr;
-  B2R_CUDA_OK(cudaMalloc(&dp, n * sizeof(float)));
-  allocs->push_back(dp);
-  B2R_CUDA_OK(cudaMemcpy(dp, h, n * sizeof(float), cudaMemcpyHostToDevice));
-  *d = static_cast<const float*>(dp);
-  return B200ROMP_OK;
-}
-
 int tc_bottleneck_prepare(const ConvParams& p, const float* w1_oihw, const float* b1, const float* w2_oihw, const float* b2,
                           const float* w3_oihw, int sm_count, TcConvPlan* plan, std::vector<void*>* allocs) {
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) {
-    set_error("conv_bottleneck_tc: cuTensorMapEncodeTiled is unavailable");
-    return B200ROMP_ECUDA;
-  }
   plan->kind = 70;
   plan->eb = 2;
   plan->cin = plan->cout = 256;
@@ -326,36 +312,24 @@ int tc_bottleneck_prepare(const ConvParams& p, const float* w1_oihw, const float
   int rc = tc_pack_weights(w1_oihw, 256, 64, 1, 64, &plan->d_wpack, allocs, kRowB, 2);   // [chunk][64 x 128 B]
   if (!rc) rc = tc_pack_weights(w2_oihw, 64, 64, 9, 64, &plan->d_wpack2, allocs, kRowB, 2);
   if (!rc) rc = tc_pack_weights(w3_oihw, 64, 256, 1, 256, &plan->d_wpack3, allocs, kRowB, 2);
-  if (!rc) rc = upload_floats(b1, 64, &plan->d_bias1, allocs);
-  if (!rc) rc = upload_floats(b2, 64, &plan->d_bias2, allocs);
   if (rc) return rc;
-  // tensor map over the NHWC input slice: dims (C, W, H, N), 64-channel x 10 x 18 halo box, OOB -> zeros
-  CUtensorMap tm;
-  const cuuint64_t gdim[4] = {256, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
-  const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * 2, (cuuint64_t)p.Win * p.in_C * 2, (cuuint64_t)p.Hin * p.Win * p.in_C * 2};
-  const cuuint32_t box[4] = {64, kHaloW, kHaloH, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * 2);
-  CUresult cr = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    set_error("conv_bottleneck_tc: cuTensorMapEncodeTiled failed with %d", (int)cr);
-    return B200ROMP_ECUDA;
-  }
-  memcpy(plan->tmap_in, &tm, sizeof(tm));
+  plan->d_bias1 = static_cast<const float*>(upload(b1, 64 * sizeof(float), allocs));
+  plan->d_bias2 = static_cast<const float*>(upload(b2, 64 * sizeof(float), allocs));
+  if (!plan->d_bias1 || !plan->d_bias2) return B200ROMP_ECUDA;
+  // the 256-channel input slice, loaded 64 channels at a time with a 10 x 18 halo box
+  rc = tc_encode_nhwc_input(&plan->tmap_in, p, 2, 64, kHaloW, kHaloH, CU_TENSOR_MAP_SWIZZLE_128B, "conv_bottleneck_tc");
+  if (rc) return rc;
   B2R_CUDA_OK(cudaFuncSetAttribute(conv_bottleneck_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   B2R_CUDA_OK(cudaFuncSetAttribute(conv_bottleneck_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   return B200ROMP_OK;
 }
 
 int tc_bottleneck_launch(const TcConvPlan& plan, const ConvParams& p, const BottleneckMids& mids, cudaStream_t stream) {
-  CUtensorMap tm;
-  memcpy(&tm, plan.tmap_in, sizeof(tm));
   const int tiles_x = p.Wout / 8, tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   const dim3 grid(std::min(plan.grid_x, num_tiles));
   auto kern = mids.t1 != nullptr || mids.t2 != nullptr ? conv_bottleneck_tc_kernel<true> : conv_bottleneck_tc_kernel<false>;
-  B2R_CUDA_OK(tc_launch(kern, grid, kBnThreads, plan.smem_bytes, stream, tm, p, reinterpret_cast<const uint8_t*>(plan.d_wpack),
+  B2R_CUDA_OK(tc_launch(kern, grid, kBnThreads, plan.smem_bytes, stream, plan.tmap_in, p, reinterpret_cast<const uint8_t*>(plan.d_wpack),
                         reinterpret_cast<const uint8_t*>(plan.d_wpack2), reinterpret_cast<const uint8_t*>(plan.d_wpack3),
                         plan.d_bias1, plan.d_bias2, mids, tiles_x, tiles_y, num_tiles));
   return B200ROMP_OK;

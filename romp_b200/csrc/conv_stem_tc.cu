@@ -190,21 +190,16 @@ int tc_stem_prepare(const ConvParams& p, const float* w_oihw, int sm_count, TcCo
 }
 
 int tc_stem_launch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream) {
-  // raw-window tensor map over the (caller-owned, re-bindable) u8 frames: [N][H][W*3 bytes], zero fill outside
-  PFN_encodeTiled encode = tc_get_encode();
-  B2R_REQUIRE(encode && (reinterpret_cast<uintptr_t>(p.in) & 15) == 0 && (p.Win * 3) % 16 == 0,
+  // raw-window tensor map over the (caller-owned, re-bindable) u8 frames: [N][H][W*3 bytes], zero fill outside.  Encoded at
+  // every launch, since the frames may be re-bound; a failure is reported as EINVAL, like the frame checks.
+  B2R_REQUIRE((reinterpret_cast<uintptr_t>(p.in) & 15) == 0 && (p.Win * 3) % 16 == 0,
               "conv_stem_tc: frames must be 16 B aligned with a row pitch that is a multiple of 16 B");
   CUtensorMap raw;
-  {
-    const cuuint64_t gdim[3] = {(cuuint64_t)p.Win * 3, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
-    const cuuint64_t gstr[2] = {(cuuint64_t)p.Win * 3, (cuuint64_t)p.Win * 3 * p.Hin};
-    const cuuint32_t box[3] = {(cuuint32_t)kRawRowB, (cuuint32_t)kRawRows, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult cr = encode(&raw, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(p.in), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B2R_REQUIRE(cr == CUDA_SUCCESS, "conv_stem_tc: cuTensorMapEncodeTiled (frames) failed with %d", (int)cr);
-  }
+  const cuuint64_t gdim[3] = {(cuuint64_t)p.Win * 3, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
+  const cuuint64_t gstr[2] = {(cuuint64_t)p.Win * 3, (cuuint64_t)p.Win * 3 * p.Hin};
+  const cuuint32_t box[3] = {(cuuint32_t)kRawRowB, (cuuint32_t)kRawRows, 1};
+  if (tc_encode_tiled(&raw, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, p.in, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_NONE, "conv_stem_tc (frames)"))
+    return B200ROMP_EINVAL;
   const int tiles_x = p.Wout / 8, tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   dim3 grid(std::min(plan.grid_x, num_tiles), 1);

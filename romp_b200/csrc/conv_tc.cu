@@ -227,6 +227,32 @@ PFN_encodeTiled tc_get_encode() {
   return fn;
 }
 
+int tc_encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                    const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* tag) {
+  PFN_encodeTiled encode = tc_get_encode();
+  if (!encode) {
+    set_error("%s: cuTensorMapEncodeTiled is unavailable", tag);
+    return B200ROMP_ECUDA;
+  }
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const CUresult cr = encode(map, dtype, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    set_error("%s: cuTensorMapEncodeTiled failed with %d", tag, (int)cr);
+    return B200ROMP_ECUDA;
+  }
+  return B200ROMP_OK;
+}
+
+int tc_encode_nhwc_input(CUtensorMap* map, const ConvParams& p, int eb, int box_c, int box_w, int box_h, CUtensorMapSwizzle swizzle,
+                         const char* tag) {
+  const cuuint64_t dims[4] = {(cuuint64_t)p.cin, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
+  const cuuint64_t strides[3] = {(cuuint64_t)p.in_C * eb, (cuuint64_t)p.Win * p.in_C * eb, (cuuint64_t)p.Hin * p.Win * p.in_C * eb};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  return tc_encode_tiled(map, eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4,
+                         static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * eb, dims, strides, box, swizzle, tag);
+}
+
 float tc_round_tf32_host(float w) {
   uint32_t u;
   memcpy(&u, &w, 4);
@@ -260,15 +286,10 @@ std::vector<uint8_t> tc_pack_image(const float* w_oihw, int cin, int cout, int t
   return img;
 }
 
-int tc_upload_image(const std::vector<uint8_t>& img, void** d_out, std::vector<void*>* allocs) {
-  B2R_CUDA_OK(cudaMalloc(d_out, img.size()));
-  allocs->push_back(*d_out);
-  B2R_CUDA_OK(cudaMemcpy(*d_out, img.data(), img.size(), cudaMemcpyHostToDevice));
-  return B200ROMP_OK;
-}
-
 int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, void** d_out, std::vector<void*>* allocs, int rowb, int eb) {
-  return tc_upload_image(tc_pack_image(w_oihw, cin, cout, taps, nt, rowb, eb), d_out, allocs);
+  const std::vector<uint8_t> img = tc_pack_image(w_oihw, cin, cout, taps, nt, rowb, eb);
+  *d_out = upload(img.data(), img.size(), allocs);
+  return *d_out ? B200ROMP_OK : B200ROMP_ECUDA;
 }
 
 std::string TcConvPlan::describe() const {
@@ -359,15 +380,11 @@ static int launch_inst(const TcConvPlan& plan, const ConvParams& p, cudaStream_t
     return B200ROMP_OK;
   }
   auto kern = p.cout % NT == 0 && tc_nhwc_out(p, p.cout) ? conv_tc_kernel<MODE, CIN, NT, EB, false> : conv_tc_kernel<MODE, CIN, NT, EB, true>;
-  CUtensorMap tm;
-  memcpy(&tm, plan.tmap_in, sizeof(tm));
-  S2Maps s2;
-  memcpy(&s2, plan.tmap_s2, sizeof(s2));
   const int tiles_x = p.Wout / 8, tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   dim3 grid(std::min(plan.grid_x, num_tiles), plan.grid_y);
-  B2R_CUDA_OK(tc_launch(kern, grid, kTcThreads, plan.smem_bytes, stream, tm, s2, p, reinterpret_cast<const uint8_t*>(plan.d_wpack), tiles_x,
-                        tiles_y, num_tiles, plan.stages, plan.kmask));
+  B2R_CUDA_OK(tc_launch(kern, grid, kTcThreads, plan.smem_bytes, stream, plan.tmap_in, plan.tmap_s2, p,
+                        reinterpret_cast<const uint8_t*>(plan.d_wpack), tiles_x, tiles_y, num_tiles, plan.stages, plan.kmask));
   return B200ROMP_OK;
 }
 
@@ -393,11 +410,6 @@ static int dispatch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t st
 
 int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_oihw, int sm_count, TcConvPlan* plan,
                     std::vector<void*>* allocs) {
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) {
-    set_error("conv_tc: cuTensorMapEncodeTiled is unavailable");
-    return B200ROMP_ECUDA;
-  }
   if (!tc_tile(p, ksize, stride, plan)) {
     set_error("conv_tc: k%d s%d cin%d does not fit shared memory", ksize, stride, p.cin);
     return B200ROMP_EINVAL;
@@ -407,7 +419,6 @@ int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_o
   plan->grid_x = std::max(1, sm_count / plan->grid_y);
   int rc = tc_pack_weights(w_oihw, p.cin, p.cout, ksize * ksize, plan->nt, &plan->d_wpack, allocs, rowb, eb);
   if (rc) return rc;
-  const CUtensorMapDataType dtype = eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   const CUtensorMapSwizzle swizzle = rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   if (stride == 2) {
     // one map per input parity over the space-to-depth view: dims ([pw*C+c], W/2, ph, H/2, N)
@@ -415,34 +426,16 @@ int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_o
     const cuuint64_t gdim[5] = {2 * C, (cuuint64_t)p.Win / 2, 2, (cuuint64_t)p.Hin / 2, (cuuint64_t)p.B};
     const cuuint64_t E = (cuuint64_t)eb;
     const cuuint64_t gstr[4] = {2 * C * E, (cuuint64_t)p.Win * C * E, 2 * (cuuint64_t)p.Win * C * E, (cuuint64_t)p.Hin * p.Win * C * E};
-    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    const CUtensorMapDataType dtype = eb == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
     for (int i = 0; i < 4; ++i) {
       const cuuint32_t box[5] = {(cuuint32_t)cw, (cuuint32_t)((i & 1) ? 8 : 9), 1, (cuuint32_t)(i < 2 ? 17 : 16), 1};
-      CUtensorMap tm;
-      CUresult cr = encode(&tm, dtype, 5, const_cast<void*>(p.in), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (cr != CUDA_SUCCESS) {
-        set_error("conv_tc: cuTensorMapEncodeTiled (stride 2) failed with %d", (int)cr);
-        return B200ROMP_ECUDA;
-      }
-      memcpy(plan->tmap_s2[i], &tm, sizeof(tm));
+      rc = tc_encode_tiled(&plan->tmap_s2.m[i], dtype, 5, p.in, gdim, gstr, box, swizzle, "conv_tc (stride 2)");
+      if (rc) return rc;
     }
   } else {
-    // tensor map over the NHWC input: dims (C slice, W, H, N), halo box, OOB -> zeros
     const int hh = 16 + 2 * (ksize / 2), hw = 8 + 2 * (ksize / 2);
-    CUtensorMap tm;
-    const cuuint64_t gdim[4] = {(cuuint64_t)p.cin, (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)p.B};
-    const cuuint64_t gstr[3] = {(cuuint64_t)p.in_C * eb, (cuuint64_t)p.Win * p.in_C * eb, (cuuint64_t)p.Hin * p.Win * p.in_C * eb};
-    const cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)hw, (cuuint32_t)hh, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    void* base = const_cast<uint8_t*>(static_cast<const uint8_t*>(p.in) + (size_t)p.in_c_off * eb);
-    CUresult cr = encode(&tm, dtype, 4, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("conv_tc: cuTensorMapEncodeTiled failed with %d", (int)cr);
-      return B200ROMP_ECUDA;
-    }
-    memcpy(plan->tmap_in, &tm, sizeof(tm));
+    rc = tc_encode_nhwc_input(&plan->tmap_in, p, eb, cw, hw, hh, swizzle, "conv_tc");
+    if (rc) return rc;
   }
   return dispatch(*plan, p, nullptr, true);
 }

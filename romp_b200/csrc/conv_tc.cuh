@@ -22,8 +22,8 @@ struct TcConvPlan {
   int grid_x = 0, grid_y = 0, stages = 0;
   int smem_bytes = 0;
   void* d_wpack = nullptr;      // weights pre-arranged as the shared-memory image (bf16, swizzled)
-  alignas(64) unsigned char tmap_in[128];     // CUtensorMap for the NHWC input tensor
-  alignas(64) unsigned char tmap_s2[4][128];  // stride-2: one map per input parity (ph,pw)
+  CUtensorMap tmap_in;          // the input tensor
+  S2Maps tmap_s2;               // stride-2: one map per input parity (ph,pw)
   // bit (tap * 2 + half) = 0 skips the MMAs of that channel half of that tap (all-zero weights of a pixel-pair folded
   // conv, see net.cu fold_pixel_pairs)
   unsigned kmask = 0xFFFFFFFFu;

@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -29,6 +30,20 @@ void set_error(const char* fmt, ...) {
   g_last_error = buf;
 }
 
+void* upload(const void* host, size_t bytes, std::vector<void*>* allocs) {
+  void* d = nullptr;
+  cudaError_t e = cudaMalloc(&d, bytes);
+  if (e == cudaSuccess) {
+    allocs->push_back(d);
+    e = cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) {
+    set_error("upload of %zu bytes failed: %s", bytes, cudaGetErrorString(e));
+    return nullptr;
+  }
+  return d;
+}
+
 struct Tensor {
   int H, W, C, dtype, nchw, external;
   void* ptr = nullptr;        // device pointer (workspace slice or bound external / constant)
@@ -37,38 +52,41 @@ struct Tensor {
   size_t frame_bytes() const { return (size_t)H * W * C * dtype_size(dtype); }
 };
 
-// The kernel that runs an op.  Sum and MaxPool are set when the op is added, WgmmaBlock by fuse_basic_blocks,
-// WgmmaBottleneck by fuse_bottlenecks; every other
-// conv is Simt until choose_kernel decides at finalize.  Generic7x7 and Deconv4x4 are the CUDA-core kernels of
-// resnet_ops.cu; a Wgmma or WgmmaBlock plan with tc.fold runs on the pixel-pair view (fold_pixel_pairs).
+// The kernel that runs an op.  Sum and MaxPool are set when the op is added, WgmmaBlock and WgmmaBottleneck by
+// fuse_chains; every other conv is Simt until choose_kernel decides at finalize.  Generic7x7 and Deconv4x4 are the
+// CUDA-core kernels of resnet_ops.cu; a Wgmma or WgmmaBlock plan with tc.fold runs on the pixel-pair view
+// (fold_pixel_pairs).
 enum class Kernel { Sum, MaxPool, Simt, Generic7x7, Deconv4x4, Wgmma, WgmmaStem, WgmmaConv1d, WgmmaBlock, WgmmaBottleneck };
+
+// one conv as added: its descriptor, OIHW fp32 weights and [cout] bias (both freed at finalize)
+struct Conv {
+  b200romp_conv_desc d;
+  std::vector<float> w, b;
+  // inside a fused op, for every conv but the last: its output is an intermediate that other ops read as well, so the
+  // fused kernel writes it and it gets a buffer
+  bool stored = false;
+};
 
 struct Op {
   Kernel kernel = Kernel::Simt;
   b200romp_sum_desc sum;
-  b200romp_conv_desc d;                // sum / maxpool: d.out / d.in mirror out / base or in, d.res = -1
-  std::vector<float> w_host, b_host;   // OIHW fp32, [cout]; freed at finalize
+  // a conv: the chain of convs the op runs, one for a plain conv and the convs it replaces for a fused one; d is then the
+  // chain as one conv (input and residual = the first conv's input, output = the last conv's).  Sum / maxpool: no parts,
+  // d.out / d.in mirror out / base or in, d.res = -1.
+  b200romp_conv_desc d;
+  std::vector<Conv> parts;
   float* d_w_simt = nullptr;           // CUDA-core kernels only: [tap][cin][coutPad]
-  float* d_bias = nullptr;             // [coutPad]
+  float* d_bias = nullptr;             // the last conv's bias, [coutPad]
   int coutPad = 0;
   TcConvPlan tc;                       // wgmma kernels: packed weights, tensor maps, tiling
   int lane = 0;                        // concurrency lane inside the captured CUDA graph (b200romp_net_set_lane)
-  // WgmmaBlock: d describes the block (in and res = x, out = y, bias = b2), w_host / b_host are conv1's, w2_host / b2_host
-  // conv2's, `mid` is the intermediate tensor that no longer gets a buffer
-  int mid = -1;
-  std::vector<float> w2_host, b2_host;
-  // WgmmaBottleneck: as WgmmaBlock for its first two convs (d.cout = 256, bias = b3), w3_host / b3_host conv3's, `mid2`
-  // conv2's output.  An intermediate that other ops read as well is stored (store_mid, store_mid2) and gets a buffer.
-  int mid2 = -1;
-  bool store_mid = false, store_mid2 = false;
-  std::vector<float> w3_host, b3_host;
 };
 
-// the tensors an op writes: its output, and a fused Bottleneck's stored intermediates
+// the tensors an op writes: its output, and a fused op's stored intermediates
 static std::vector<int> op_outputs(const Op& op) {
   std::vector<int> o{op.d.out};
-  if (op.store_mid) o.push_back(op.mid);
-  if (op.store_mid2) o.push_back(op.mid2);
+  for (size_t k = 0; k + 1 < op.parts.size(); ++k)
+    if (op.parts[k].stored) o.push_back(op.parts[k].d.out);
   return o;
 }
 
@@ -229,22 +247,22 @@ int b200romp_net_add_const_tensor(b200romp_net* net, int H, int W, int C, int dt
   Tensor& t = net->tensors[id];
   t.constant = true;
   B2R_CUDA_OK(cudaSetDevice(net->device));
-  B2R_CUDA_OK(cudaMalloc(&t.ptr, t.frame_bytes()));
-  net->device_allocs.push_back(t.ptr);
-  B2R_CUDA_OK(cudaMemcpy(t.ptr, host_data, t.frame_bytes(), cudaMemcpyHostToDevice));
-  return id;
+  t.ptr = upload(host_data, t.frame_bytes(), &net->device_allocs);
+  return t.ptr ? id : B200ROMP_ECUDA;
 }
 
 int b200romp_net_add_conv(b200romp_net* net, const b200romp_conv_desc* desc, const float* weight, const float* bias) {
   B2R_REQUIRE(net && !net->finalized && desc && weight, "add_conv: bad arguments");
   int rc = validate_desc(net->tensors, *desc);
   if (rc) return rc;
+  Conv c;
+  c.d = *desc;
+  c.w.assign(weight, weight + (size_t)desc->cout * desc->cin * conv_taps(desc->ksize));
+  c.b.assign(desc->cout, 0.f);
+  if (bias) c.b.assign(bias, bias + desc->cout);
   Op op;
   op.d = *desc;
-  const size_t nw = (size_t)desc->cout * desc->cin * conv_taps(desc->ksize);
-  op.w_host.assign(weight, weight + nw);
-  op.b_host.assign(desc->cout, 0.f);
-  if (bias) op.b_host.assign(bias, bias + desc->cout);
+  op.parts.push_back(std::move(c));
   net->ops.push_back(std::move(op));
   return (int)net->ops.size() - 1;
 }
@@ -342,25 +360,18 @@ static int enqueue_op(b200romp_net* net, Op& op, int batch, cudaStream_t stream)
     case Kernel::WgmmaBlock: return tc_block_launch(op.tc, p, stream);
     case Kernel::WgmmaBottleneck: {
       BottleneckMids mids;
-      if (op.store_mid) {
-        mids.t1 = static_cast<__nv_bfloat16*>(net->tensors[op.mid].ptr);
-        mids.t1_C = net->tensors[op.mid].C;
-      }
-      if (op.store_mid2) {
-        mids.t2 = static_cast<__nv_bfloat16*>(net->tensors[op.mid2].ptr);
-        mids.t2_C = net->tensors[op.mid2].C;
-      }
+      auto mid = [&](int k, int* C) -> __nv_bfloat16* {
+        if (!op.parts[k].stored) return nullptr;
+        const Tensor& t = net->tensors[op.parts[k].d.out];
+        *C = t.C;
+        return static_cast<__nv_bfloat16*>(t.ptr);
+      };
+      mids.t1 = mid(0, &mids.t1_C);
+      mids.t2 = mid(1, &mids.t2_C);
       return tc_bottleneck_launch(op.tc, p, mids, stream);
     }
   }
   return B200ROMP_EINVAL;
-}
-
-static int upload(b200romp_net* net, const std::vector<float>& v, float** d) {
-  B2R_CUDA_OK(cudaMalloc(d, v.size() * sizeof(float)));
-  net->device_allocs.push_back(*d);
-  B2R_CUDA_OK(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return B200ROMP_OK;
 }
 
 // Pixel-pair folding of a 32->32 3x3 stride-1 conv.  With N = Cout = 32 every MMA still fetches a
@@ -415,11 +426,6 @@ static unsigned fold_kmask() {
   return m;
 }
 
-// HRNet BasicBlocks relu(conv2(relu(conv1(x))) + x) whose convs are 3x3 stride-1 64->64 (or pixel-pair foldable 32->32) bf16
-// layers become one op on the fused block kernel (conv_block_tc.cu): the intermediate never reaches HBM and x is read once.
-// Ops i, i+1 fuse when conv2 reads exactly conv1's output, that tensor is internal and read by nothing else, conv2's
-// residual is conv1's input slice, and the block kernel supports the fused op.  A caller that binds the intermediate as an
-// external tensor keeps the two convs.
 // a bf16 NHWC stride-1 ReLU conv of kernel size `ksize` from cin to cout channels that a fused wgmma kernel may take
 static bool is_bf16_relu_conv(const b200romp_net* net, const Op& op, int ksize, int cin, int cout) {
   const b200romp_conv_desc& d = op.d;
@@ -428,10 +434,6 @@ static bool is_bf16_relu_conv(const b200romp_net* net, const Op& op, int ksize, 
   return d.ksize == ksize && d.stride == 1 && d.upsample == 1 && d.relu && !d.input_norm && d.pow_channel < 0 &&
          (d.engine == B200ROMP_ENGINE_AUTO || d.engine == B200ROMP_ENGINE_WGMMA) && ti.dtype == B200ROMP_BF16 &&
          to.dtype == B200ROMP_BF16 && !to.nchw && d.cin == cin && d.cout == cout;
-}
-
-static bool is_bf16_block_conv(const b200romp_net* net, const Op& op) {
-  return is_bf16_relu_conv(net, op, 3, 64, 64) || is_bf16_relu_conv(net, op, 3, 32, 32);
 }
 
 // how many ops read / write each tensor
@@ -456,104 +458,71 @@ static bool fusable_intermediate(const b200romp_net* net, const Op& a, const Op&
          writes[t] == 1 && b.d.res != t;
 }
 
-static void fuse_basic_blocks(b200romp_net* net) {
-  std::vector<int> reads, writes;
-  count_accesses(net, &reads, &writes);
-  std::vector<Op> fused;
-  fused.reserve(net->ops.size());
-  for (size_t i = 0; i < net->ops.size(); ++i) {
-    Op& a = net->ops[i];
-    if (i + 1 < net->ops.size()) {
-      Op& b = net->ops[i + 1];
-      const int x = a.d.in, t = a.d.out;
-      const Tensor& tt = net->tensors[t];
-      const int C = a.d.cin;
-      bool ok = is_bf16_block_conv(net, a) && is_bf16_block_conv(net, b) && a.d.res < 0 && b.d.cin == C && a.lane == b.lane &&
-                b.d.in == t && b.d.in_c_off == 0 && a.d.out_c_off == 0 && tt.C == C && !tt.external && !tt.constant &&
-                reads[t] == 1 && writes[t] == 1 && b.d.res == x && b.d.res_c_off == a.d.in_c_off && !b.d.res_broadcast &&
-                !net->tensors[x].external && !net->tensors[b.d.out].external &&
-                (C == 64 || (fold_eligible(net, a) && fold_eligible(net, b)));   // the 32-channel kernel is the folded 64-channel one
-      if (ok) {
-        Op f;
-        f.kernel = Kernel::WgmmaBlock;
-        f.d = a.d;
-        f.d.out = b.d.out;
-        f.d.out_c_off = b.d.out_c_off;
-        f.d.res = x;
-        f.d.res_c_off = b.d.res_c_off;
-        f.tc.fold = C == 32;
-        ConvParams p;
-        fill_params(net, f, 1, true, &p);
-        if (tc_block_supported(p, f.tc.fold)) {
-          f.mid = t;
-          f.lane = a.lane;
-          f.w_host = std::move(a.w_host);
-          f.b_host = std::move(a.b_host);
-          f.w2_host = std::move(b.w_host);
-          f.b2_host = std::move(b.b_host);
-          fused.push_back(std::move(f));
-          ++i;
-          continue;
-        }
-      }
-    }
-    fused.push_back(std::move(a));
-  }
-  net->ops = std::move(fused);
-}
+// A run of consecutive convs that one fused wgmma kernel takes as a single op, the intermediates kept on chip and the input
+// read once:
+//  - HRNet BasicBlocks relu(conv2(relu(conv1(x))) + x) of 3x3 64->64 convs, or of pixel-pair foldable 32->32 ones, on the
+//    block kernel (conv_block_tc.cu);
+//  - ResNet Bottlenecks relu(conv3(relu(conv2(relu(conv1(x))))) + x) of 1x1 256->64, 3x3 64->64 and 1x1 64->256 convs (HRNet
+//    layer1.1 .. layer1.3) on the Bottleneck kernel (conv_bottleneck_tc.cu).
+struct ChainPattern {
+  Kernel kernel;
+  std::vector<std::array<int, 3>> convs;   // (ksize, cin, cout) of each conv of the chain
+  bool fold;                               // the kernel runs on the pixel-pair view: every conv must be fold-eligible
+  bool shared_mids;                        // an intermediate may have other readers; the kernel then stores it
+  bool (*supported)(const ConvParams& p, bool fold);
+};
 
-// ResNet Bottlenecks relu(conv3(relu(conv2(relu(conv1(x))))) + x) with identity residual, 1x1 256->64, 3x3 stride-1 64->64 and
-// 1x1 64->256 bf16 convs (HRNet layer1.1 .. layer1.3), become one op on the fused Bottleneck kernel (conv_bottleneck_tc.cu):
-// the two 64-channel intermediates never reach HBM and x is read once.  Ops i, i+1, i+2 fuse when each intermediate is
-// internal and written only by its conv, conv3's residual is conv1's input slice, the three run on one lane, and the
-// Bottleneck kernel supports the fused op.  An intermediate that later ops read as well is also written by the kernel.
-static void fuse_bottlenecks(b200romp_net* net) {
+// Replaces every run of ops that matches `pat` by one op.  Ops i .. i+n-1 fuse when each is a conv as added, of the
+// pattern's shape, and all run on one lane; each intermediate is fusable (fusable_intermediate) and, unless the pattern
+// shares them, read by nothing else; only the last conv adds a residual, and that is the first conv's input slice; the
+// chain's input and output are internal; and the kernel supports the fused op.  A caller that binds an intermediate as an
+// external tensor keeps the convs.
+static void fuse_chains(b200romp_net* net, const ChainPattern& pat) {
   std::vector<int> reads, writes;
   count_accesses(net, &reads, &writes);
+  const size_t n = pat.convs.size();
   std::vector<Op> fused;
   fused.reserve(net->ops.size());
   for (size_t i = 0; i < net->ops.size(); ++i) {
-    Op& a = net->ops[i];
-    if (i + 2 < net->ops.size()) {
-      Op& b = net->ops[i + 1];
-      Op& c = net->ops[i + 2];
-      const int x = a.d.in;
-      const bool ok = a.kernel == Kernel::Simt && b.kernel == Kernel::Simt && c.kernel == Kernel::Simt &&
-                      is_bf16_relu_conv(net, a, 1, 256, 64) && is_bf16_relu_conv(net, b, 3, 64, 64) &&
-                      is_bf16_relu_conv(net, c, 1, 64, 256) && a.d.res < 0 && b.d.res < 0 && a.lane == b.lane &&
-                      b.lane == c.lane && fusable_intermediate(net, a, b, writes) && fusable_intermediate(net, b, c, writes) &&
-                      c.d.res == x && c.d.res_c_off == a.d.in_c_off &&
-                      !c.d.res_broadcast && !net->tensors[x].external && !net->tensors[c.d.out].external;
-      if (ok) {
-        Op f;
-        f.kernel = Kernel::WgmmaBottleneck;
-        f.d = a.d;
-        f.d.cout = c.d.cout;
-        f.d.out = c.d.out;
-        f.d.out_c_off = c.d.out_c_off;
-        f.d.res = x;
-        f.d.res_c_off = c.d.res_c_off;
-        ConvParams p;
-        fill_params(net, f, 1, true, &p);
-        if (tc_bottleneck_supported(p)) {
-          f.mid = a.d.out;
-          f.mid2 = b.d.out;
-          f.store_mid = reads[f.mid] > 1;
-          f.store_mid2 = reads[f.mid2] > 1;
-          f.lane = a.lane;
-          f.w_host = std::move(a.w_host);
-          f.b_host = std::move(a.b_host);
-          f.w2_host = std::move(b.w_host);
-          f.b2_host = std::move(b.b_host);
-          f.w3_host = std::move(c.w_host);
-          f.b3_host = std::move(c.b_host);
-          fused.push_back(std::move(f));
-          i += 2;
-          continue;
+    Op* c = &net->ops[i];
+    bool ok = i + n <= net->ops.size();
+    for (size_t k = 0; ok && k < n; ++k) {
+      const std::array<int, 3>& s = pat.convs[k];
+      ok = c[k].kernel == Kernel::Simt && is_bf16_relu_conv(net, c[k], s[0], s[1], s[2]) && c[k].lane == c[0].lane &&
+           (!pat.fold || fold_eligible(net, c[k]));
+      if (ok && k + 1 < n)
+        ok = c[k].d.res < 0 && fusable_intermediate(net, c[k], c[k + 1], writes) && (pat.shared_mids || reads[c[k].d.out] == 1);
+    }
+    if (ok) {
+      const b200romp_conv_desc& first = c[0].d;
+      const b200romp_conv_desc& last = c[n - 1].d;
+      ok = last.res == first.in && last.res_c_off == first.in_c_off && !last.res_broadcast &&
+           !net->tensors[first.in].external && !net->tensors[last.out].external;
+    }
+    if (ok) {
+      Op f;
+      f.kernel = pat.kernel;
+      f.d = c[0].d;
+      f.d.cout = c[n - 1].d.cout;
+      f.d.out = c[n - 1].d.out;
+      f.d.out_c_off = c[n - 1].d.out_c_off;
+      f.d.res = c[0].d.in;
+      f.d.res_c_off = c[n - 1].d.res_c_off;
+      f.tc.fold = pat.fold;
+      f.lane = c[0].lane;
+      ConvParams p;
+      fill_params(net, f, 1, true, &p);
+      if (pat.supported(p, pat.fold)) {
+        for (size_t k = 0; k < n; ++k) {
+          f.parts.push_back(std::move(c[k].parts[0]));
+          f.parts.back().stored = k + 1 < n && reads[c[k].d.out] > 1;
         }
+        fused.push_back(std::move(f));
+        i += n - 1;
+        continue;
       }
     }
-    fused.push_back(std::move(a));
+    fused.push_back(std::move(net->ops[i]));
   }
   net->ops = std::move(fused);
 }
@@ -596,20 +565,20 @@ static int choose_kernel(const b200romp_net* net, int i, Op& op) {
 // Uploads what op's kernel reads and builds its plan.  Every conv gets its bias zero-padded to a multiple of 64 (the wgmma
 // epilogues read up to grid_y * NT); only the CUDA-core kernels get the [tap][cin][coutPad] fp32 weights.
 static int prepare_op(b200romp_net* net, Op& op) {
-  if (op.kernel == Kernel::Sum || op.kernel == Kernel::MaxPool) return B200ROMP_OK;
+  if (op.parts.empty()) return B200ROMP_OK;   // sum, maxpool
   const b200romp_conv_desc& d = op.d;
-  std::vector<float> w = std::move(op.w_host), b = std::move(op.b_host), w2 = std::move(op.w2_host), b2 = std::move(op.b2_host);
-  if (op.tc.fold) {
-    fold_pixel_pairs(&w, &b);
-    if (op.kernel == Kernel::WgmmaBlock) fold_pixel_pairs(&w2, &b2);
+  // the parts' host weights, freed on return
+  std::vector<std::vector<float>> w, b;
+  for (Conv& c : op.parts) {
+    w.push_back(std::move(c.w));
+    b.push_back(std::move(c.b));
+    if (op.tc.fold) fold_pixel_pairs(&w.back(), &b.back());
   }
-  std::vector<float> b3 = std::move(op.b3_host);
-  // a block's bias is conv2's, a Bottleneck's conv3's
-  std::vector<float> bias = op.kernel == Kernel::WgmmaBlock ? b2 : op.kernel == Kernel::WgmmaBottleneck ? b3 : b;
+  std::vector<float> bias = b.back();
   op.coutPad = ((int)bias.size() + 63) / 64 * 64;
   bias.resize(op.coutPad, 0.f);
-  int rc = upload(net, bias, &op.d_bias);
-  if (rc) return rc;
+  op.d_bias = static_cast<float*>(upload(bias.data(), bias.size() * sizeof(float), &net->device_allocs));
+  if (!op.d_bias) return B200ROMP_ECUDA;
   ConvParams p;
   fill_params(net, op, net->max_batch, true, &p);
   switch (op.kernel) {
@@ -622,19 +591,20 @@ static int prepare_op(b200romp_net* net, Op& op) {
         for (int ci = 0; ci < d.cin; ++ci)
           for (int t = 0; t < taps; ++t)   // conv: OIHW; ConvTranspose2d (code 42): PyTorch's [cin][cout][4][4]
             packed[((size_t)t * d.cin + ci) * op.coutPad + co] =
-                d.ksize == 42 ? w[((size_t)ci * d.cout + co) * taps + t] : w[((size_t)co * d.cin + ci) * taps + t];
-      return upload(net, packed, &op.d_w_simt);
+                d.ksize == 42 ? w[0][((size_t)ci * d.cout + co) * taps + t] : w[0][((size_t)co * d.cin + ci) * taps + t];
+      op.d_w_simt = static_cast<float*>(upload(packed.data(), packed.size() * sizeof(float), &net->device_allocs));
+      return op.d_w_simt ? B200ROMP_OK : B200ROMP_ECUDA;
     }
     case Kernel::Wgmma:
       if (op.tc.fold) op.tc.kmask = fold_kmask();
-      return tc_conv_prepare(p, d.ksize, d.stride, w.data(), net->sm_count, &op.tc, &net->device_allocs);
-    case Kernel::WgmmaStem: return tc_stem_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
-    case Kernel::WgmmaConv1d: return tc_conv1d_prepare(p, w.data(), net->sm_count, &op.tc, &net->device_allocs);
-    case Kernel::WgmmaBlock: return tc_block_prepare(p, w.data(), b.data(), w2.data(), net->sm_count, &op.tc, &net->device_allocs);
-    case Kernel::WgmmaBottleneck: {
-      const std::vector<float> w3 = std::move(op.w3_host);
-      return tc_bottleneck_prepare(p, w.data(), b.data(), w2.data(), b2.data(), w3.data(), net->sm_count, &op.tc, &net->device_allocs);
-    }
+      return tc_conv_prepare(p, d.ksize, d.stride, w[0].data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaStem: return tc_stem_prepare(p, w[0].data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaConv1d: return tc_conv1d_prepare(p, w[0].data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaBlock:
+      return tc_block_prepare(p, w[0].data(), b[0].data(), w[1].data(), net->sm_count, &op.tc, &net->device_allocs);
+    case Kernel::WgmmaBottleneck:
+      return tc_bottleneck_prepare(p, w[0].data(), b[0].data(), w[1].data(), b[1].data(), w[2].data(), net->sm_count, &op.tc,
+                                   &net->device_allocs);
     default: return B200ROMP_OK;
   }
 }
@@ -642,8 +612,11 @@ static int prepare_op(b200romp_net* net, Op& op) {
 int b200romp_net_finalize(b200romp_net* net, int max_batch) {
   B2R_REQUIRE(net && !net->finalized && max_batch > 0, "finalize: bad arguments");
   B2R_CUDA_OK(cudaSetDevice(net->device));
-  fuse_basic_blocks(net);   // before liveness: a fused block's intermediate gets no buffer
-  fuse_bottlenecks(net);    // likewise a fused Bottleneck's two, unless other ops read them
+  // before liveness: a fused op's intermediates get no buffer unless other ops read them
+  fuse_chains(net, {Kernel::WgmmaBlock, {{3, 64, 64}, {3, 64, 64}}, false, false, tc_block_supported});
+  fuse_chains(net, {Kernel::WgmmaBlock, {{3, 32, 32}, {3, 32, 32}}, true, false, tc_block_supported});   // folded to 64
+  fuse_chains(net, {Kernel::WgmmaBottleneck, {{1, 256, 64}, {3, 64, 64}, {1, 64, 256}}, false, true,
+                    [](const ConvParams& p, bool) { return tc_bottleneck_supported(p); }});
   const int nT = (int)net->tensors.size(), nO = (int)net->ops.size();
   // ---- liveness over the linear op order
   for (int i = 0; i < nO; ++i) {
@@ -887,6 +860,15 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
   if (!net || !buf || len <= 0) return B200ROMP_EINVAL;
   std::string s;
   char line[384];
+  // the line of one conv; `bracket` describes the kernel that runs it
+  auto conv_line = [&](size_t i, const b200romp_conv_desc& d, Kernel kernel, const char* bracket) {
+    const Tensor& ti = net->tensors[d.in];
+    const Tensor& to = net->tensors[d.out];
+    snprintf(line, sizeof(line), "op%03zu %s k%d s%d %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up%d relu%d%s\n", i,
+             on_wgmma(kernel) ? "wgmma  " : "simt   ", d.ksize, d.stride, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, d.out,
+             to.H, to.W, to.C, d.out_c_off, d.res, d.upsample, d.relu, bracket);
+    s += line;
+  };
   for (size_t i = 0; i < net->ops.size(); ++i) {
     const Op& op = net->ops[i];
     const b200romp_conv_desc& d = op.d;
@@ -895,43 +877,36 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
     switch (op.kernel) {
       case Kernel::MaxPool:
         snprintf(line, sizeof(line), "op%03zu maxpool 3x3 s2 in t%d[%dx%dx%d] out t%d[%dx%dx%d]\n", i, d.in, ti.H, ti.W, ti.C, d.out, to.H, to.W, to.C);
+        s += line;
         break;
       case Kernel::Sum: {
         int n = snprintf(line, sizeof(line), "op%03zu sum     out t%d[%dx%dx%d] = relu%d( t%d", i, op.sum.out, to.H, to.W, to.C, op.sum.relu, op.sum.base);
         for (int k = 0; k < op.sum.n_terms; ++k) n += snprintf(line + n, sizeof(line) - n, " + up%d(t%d)", op.sum.up[k], op.sum.term[k]);
         snprintf(line + n, sizeof(line) - n, " )\n");
+        s += line;
         break;
       }
       case Kernel::WgmmaBlock: {   // one launch, two convs: a folded block runs both of them on pixel pairs
-        const Tensor& tm = net->tensors[op.mid];
+        const int mid = op.parts[0].d.out;
+        const Tensor& tm = net->tensors[mid];
         snprintf(line, sizeof(line),
                  "op%03zu wgmma   block k3 s1 %d->%d->%d in t%d[%dx%dx%d]+%d mid t%d[%dx%dx%d] out t%d[%dx%dx%d]+%d res t%d+%d up1 relu1 "
                  "bias1 bias2 [tc-block grid %d smem %d%s]\n",
-                 i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
+                 i, d.cin, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, mid, tm.H, tm.W, tm.C, d.out, to.H, to.W, to.C,
                  d.out_c_off, d.res, d.res_c_off, op.tc.grid_x, op.tc.smem_bytes, op.tc.fold ? " conv1 pixel-pairs conv2 pixel-pairs" : "");
+        s += line;
         break;
       }
-      case Kernel::WgmmaBottleneck: {   // one launch, three convs: one line per conv, all with the op's number
-        const Tensor& tm = net->tensors[op.mid];
-        const Tensor& tm2 = net->tensors[op.mid2];
-        const char* fmt = "op%03zu wgmma   k%d s1 %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up1 relu1 "
-                          "[tc-bottleneck conv%d of k1-k3-k1 grid %d smem %d]\n";
-        snprintf(line, sizeof(line), fmt, i, 1, d.cin, tm.C, d.in, ti.H, ti.W, ti.C, d.in_c_off, op.mid, tm.H, tm.W, tm.C, 0, -1, 1,
-                 op.tc.grid_x, op.tc.smem_bytes);
-        s += line;
-        snprintf(line, sizeof(line), fmt, i, 3, tm.C, tm2.C, op.mid, tm.H, tm.W, tm.C, 0, op.mid2, tm2.H, tm2.W, tm2.C, 0, -1, 2,
-                 op.tc.grid_x, op.tc.smem_bytes);
-        s += line;
-        snprintf(line, sizeof(line), fmt, i, 1, tm2.C, d.cout, op.mid2, tm2.H, tm2.W, tm2.C, 0, d.out, to.H, to.W, to.C, d.out_c_off,
-                 d.res, 3, op.tc.grid_x, op.tc.smem_bytes);
+      case Kernel::WgmmaBottleneck:   // one launch, three convs: one line per conv, all with the op's number
+        for (size_t k = 0; k < op.parts.size(); ++k) {
+          char bracket[96];
+          snprintf(bracket, sizeof(bracket), " [tc-bottleneck conv%zu of k1-k3-k1 grid %d smem %d]", k + 1, op.tc.grid_x, op.tc.smem_bytes);
+          conv_line(i, op.parts[k].d, op.kernel, bracket);
+        }
         break;
-      }
       default:
-        snprintf(line, sizeof(line), "op%03zu %s k%d s%d %4d->%-4d in t%d[%dx%dx%d]+%d out t%d[%dx%dx%d]+%d res t%d up%d relu%d%s\n", i,
-                 on_wgmma(op.kernel) ? "wgmma  " : "simt   ", d.ksize, d.stride, d.cin, d.cout, d.in, ti.H, ti.W, ti.C, d.in_c_off, d.out,
-                 to.H, to.W, to.C, d.out_c_off, d.res, d.upsample, d.relu, on_wgmma(op.kernel) ? op.tc.describe().c_str() : "");
+        conv_line(i, d, op.kernel, on_wgmma(op.kernel) ? op.tc.describe().c_str() : "");
     }
-    s += line;
   }
   snprintf(line, sizeof(line), "workspace %.1f MiB for max_batch %d\n", net->workspace_bytes / 1048576.0, net->max_batch);
   s += line;

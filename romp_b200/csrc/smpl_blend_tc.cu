@@ -153,31 +153,18 @@ smpl_blend_tc_kernel(const __grid_constant__ BlendMaps maps, const float* __rest
 // [81][capacity][256], coordinate-tile major
 int smpl_blend_tc_launch(const void* a_rows, int row_stride_bytes, int capacity, const void* b_rows /*fp16 [20736][448]*/,
                          float* v_posed, const float* v_template_pad, int n, const int* d_count, int sm_count, cudaStream_t stream) {
-  PFN_encodeTiled encode = tc_get_encode();
-  if (!encode) { set_error("smpl_blend_tc: cuTensorMapEncodeTiled is unavailable"); return B200ROMP_ECUDA; }
+  BlendMaps m;
+  const cuuint32_t box[2] = {32, 128};
+  const cuuint64_t a_dim[2] = {(cuuint64_t)kBlK, (cuuint64_t)capacity}, a_str[1] = {(cuuint64_t)row_stride_bytes};
+  const cuuint64_t b_dim[2] = {(cuuint64_t)kBlK, (cuuint64_t)kBlCols}, b_str[1] = {(cuuint64_t)kBlK * 2};
+  const CUtensorMapDataType f16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  int rc = tc_encode_tiled(&m.a, f16, 2, a_rows, a_dim, a_str, box, CU_TENSOR_MAP_SWIZZLE_64B, "smpl_blend_tc (A')");
+  if (!rc) rc = tc_encode_tiled(&m.b, f16, 2, b_rows, b_dim, b_str, box, CU_TENSOR_MAP_SWIZZLE_64B, "smpl_blend_tc (B')");
+  if (rc) return rc;
   static bool attr_set = false;
   if (!attr_set) {
     B2R_CUDA_OK(cudaFuncSetAttribute(smpl_blend_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlendSmem));
     attr_set = true;
-  }
-  BlendMaps m;
-  const cuuint32_t estr[2] = {1, 1};
-  const cuuint32_t box[2] = {32, 128};
-  {
-    const cuuint64_t gdim[2] = {(cuuint64_t)kBlK, (cuuint64_t)capacity};
-    const cuuint64_t gstr[1] = {(cuuint64_t)row_stride_bytes};
-    if (encode(&m.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(a_rows), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-      set_error("smpl_blend_tc: tensor map (A') failed"); return B200ROMP_ECUDA;
-    }
-  }
-  {
-    const cuuint64_t gdim[2] = {(cuuint64_t)kBlK, (cuuint64_t)kBlCols};
-    const cuuint64_t gstr[1] = {(cuuint64_t)kBlK * 2};
-    if (encode(&m.b, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(b_rows), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-      set_error("smpl_blend_tc: tensor map (B') failed"); return B200ROMP_ECUDA;
-    }
   }
   // `n` is the host-side upper bound of the person count (the device count may be smaller: surplus CTAs exit at once).
   // Few person tiles: split the coordinate tiles over more CTAs so that every SM has work.

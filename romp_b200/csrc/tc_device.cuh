@@ -371,10 +371,17 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 PFN_encodeTiled tc_get_encode();
+// A tiled TMA map over a `rank`-dimensional tensor at `base`: element dims, byte strides of dims 1 .. rank-1, box, element
+// strides 1, 128 B L2 promotion, zeros outside the tensor.  On failure the error text starts with `tag`.
+int tc_encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                    const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* tag);
+// the map over the NHWC input channel slice [in_c_off, in_c_off + cin) of `p` in bf16 (eb = 2) or fp32 (eb = 4): dims
+// (cin, W, H, N) and a (box_c, box_w, box_h, 1) halo box whose out-of-bounds pixels read as zeros
+int tc_encode_nhwc_input(CUtensorMap* map, const ConvParams& p, int eb, int box_c, int box_w, int box_h, CUtensorMapSwizzle swizzle,
+                         const char* tag);
 // bf16 / TF32 weight slab in shared-memory-image order [ntile][tap][chunk][NT rows x ROWB] with the TMA / wgmma XOR swizzle:
-// tc_pack_image builds it on the host, tc_upload_image copies an image to a new device allocation, tc_pack_weights does both
+// tc_pack_image builds it on the host, tc_pack_weights uploads it as well
 std::vector<uint8_t> tc_pack_image(const float* w_oihw, int cin, int cout, int taps, int nt, int rowb, int eb);
-int tc_upload_image(const std::vector<uint8_t>& img, void** d_out, std::vector<void*>* allocs);
 int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, void** d_out, std::vector<void*>* allocs, int rowb, int eb);
 float tc_round_tf32_host(float w);   // fp32 -> TF32, ties away from zero (cvt.rna.tf32.f32)
 
