@@ -350,6 +350,33 @@ int b200romp_bev_track_step(b200romp_bev_tracker* tracker, int batch, int capaci
                             int* d_status, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * ROMP's video mode for batches (ROMP.forward_video, -t/--temporal_optimize): the association and One-Euro smoothing of
+ * ROMP.forward's per-frame temporal path (romp_b200/temporal.py TemporalState + b200romp_one_euro_smooth), decision for
+ * decision, as ONE kernel per batch between b200romp_parse and SMPL.  The handle holds, in device memory, up to
+ * max_signals (1..16) signals, each with its tracker (NearestCenterTracker: nearest live track strictly within 200 px of
+ * cam[:,[2,1]] * 512, ties to the earliest track, drop after 30 unmatched frames, ids from 1) and its block of 64
+ * filter slots; it shares nothing with b200romp_tracks.
+ *
+ * b200romp_romp_track_step walks the frames 0..batch-1 in order over the parse's rows [0, min(*d_count, capacity))
+ * grouped by frame (batch_ids, cam [3], thetas [72], betas [10]; at most 64 rows per frame).  signal_code: device int32
+ * [batch], one code per distinct signal.  A frame without rows does nothing.  A new code takes the lowest free block
+ * (evicting the earliest registered signal when all are in use) and resets it.  Per input row: out_slot = filter slot
+ * (signal block * 64 + k, or -1 = unsmoothed) and out_track_ids (0 with show_largest).  Output rows, smoothed with freq:
+ *   show_largest == 0: one per input row, in place of it (out_batch_ids = batch_ids, *d_out_count = the row count);
+ *   show_largest != 0: one per frame with rows, the largest cam[:,0] (first on ties), in frame order (out_batch_ids =
+ *   frame, *d_out_count = frames with rows).
+ * out_thetas [.,72] / out_betas [.,10] / out_cam [.,3] must not alias the inputs (thetas keeps the unsmoothed values). */
+typedef struct b200romp_romp_tracker b200romp_romp_tracker;
+b200romp_romp_tracker* b200romp_romp_tracker_create(int device, int max_signals);
+void b200romp_romp_tracker_destroy(b200romp_romp_tracker* tracker);
+/* forget every signal, track and filter (a new video) */
+int b200romp_romp_tracker_reset(b200romp_romp_tracker* tracker, b200romp_stream stream);
+int b200romp_romp_track_step(b200romp_romp_tracker* tracker, int batch, int capacity, const int* d_count, const long long* batch_ids,
+                             const float* cam, const float* thetas, const float* betas, const int* signal_code, int show_largest,
+                             float smooth_coeff, float freq, int* d_out_count, long long* out_batch_ids, float* out_thetas,
+                             float* out_betas, float* out_cam, int* out_slot, int* out_track_ids, b200romp_stream stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Frame-sharded multi-GPU collection (SURVEY 8e; the reference's DataParallel bookkeeping it stands in for:
  * romp/lib/maps_utils/result_parser.py:59-64,123-124).  Packs the per-person output arrays of one rank into the
  * fixed-width record buffer that a single NCCL all-gather ships:

@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "lib", "libb200romp.so")
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "resnet_ops.cu"]
+SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "romp_track.cu", "resnet_ops.cu"]
 
 F32, BF16, U8 = 0, 1, 2
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_WGMMA, ENGINE_TF32 = 0, 1, 2, 3
@@ -167,6 +167,10 @@ def load():
     _sig(lib.b200romp_bev_tracker_destroy, None, vp)
     _sig(lib.b200romp_bev_tracker_reset, i32, vp, i32, vp)
     _sig(lib.b200romp_bev_track_step, i32, vp, i32, i32, *([vp] * 9), i32, f32, i32, *([vp] * 12))
+    _sig(lib.b200romp_romp_tracker_create, vp, i32, i32)
+    _sig(lib.b200romp_romp_tracker_destroy, None, vp)
+    _sig(lib.b200romp_romp_tracker_reset, i32, vp, vp)
+    _sig(lib.b200romp_romp_track_step, i32, vp, i32, i32, *([vp] * 6), i32, f32, f32, *([vp] * 7), vp)
     _sig(lib.b200romp_preprocess_bgr, i32, vp, i32, i32, i32, i32, vp, fp, vp)
     _sig(lib.b200romp_preprocess_bgr_batch, i32, C.POINTER(vp), ip, ip, ip, i32, i32, vp, vp, vp)
     _sig(lib.b200romp_pack_rows, i32, C.POINTER(vp), ip, i32, vp, i32, i32, i32, i32, vp, i32, vp)
@@ -199,4 +203,5 @@ EXPORTS = [
     "b200romp_tracks_create", "b200romp_tracks_destroy",
     "b200romp_tracks_reset", "b200romp_one_euro_smooth",
     "b200romp_bev_tracker_create", "b200romp_bev_tracker_destroy", "b200romp_bev_tracker_reset", "b200romp_bev_track_step",
+    "b200romp_romp_tracker_create", "b200romp_romp_tracker_destroy", "b200romp_romp_tracker_reset", "b200romp_romp_track_step",
 ]

@@ -236,6 +236,12 @@ class ROMP(torch.nn.Module):
                 raise RuntimeError("b200romp_tracks_create: " + self.lib.b200romp_last_error().decode())
             self._slot_host = torch.zeros(self.cap, dtype=torch.int32).pin_memory()
             self._slot_dev = torch.zeros(self.cap, dtype=torch.int32, device=self.tdevice)
+            # forward_video's device tracker: its own signals, tracks and filters (csrc/romp_track.cu)
+            self._rtrack = self.lib.b200romp_romp_tracker_create(self.device_index, self.temporal.max_signals)
+            if not self._rtrack:
+                raise RuntimeError("b200romp_romp_tracker_create: " + self.lib.b200romp_last_error().decode())
+            self._signal_codes = {}          # signal_ID -> int32 code of the device tracker
+            self._temporal_user = None       # "forward" / "video": which path holds the tracker state
 
     # ------------------------------------------------------------------------------------------
     def _net(self, in_dtype):
@@ -310,27 +316,29 @@ class ROMP(torch.nn.Module):
                                       _ptr(b["betas"]), _ptr(b["center_preds"]), _ptr(sh["parse_ws"]), sp), "parse")
 
     @torch.no_grad()
-    def run_smpl_project(self, cap, offsets, slot=None, count_on_device=True):
+    def run_smpl_project(self, cap, offsets, slot=None, count_on_device=True, rows=None):
         """Seams S3-S4 for up to ``cap`` persons (the device-side count limits it further unless count_on_device=False).
-        ``offsets``: one pad info [top,bottom,left,right,h,w] for every frame, or a device [B,6] table with one row per frame."""
+        ``offsets``: one pad info [top,bottom,left,right,h,w] for every frame, or a device [B,6] table with one row per frame.
+        ``rows``: the input rows (count, batch_ids, thetas, betas, cam) when they are not the slot's parse outputs."""
         sh, lib, sp = self.shared, self.lib, C.c_void_p(self.stream.cuda_stream)
         b = (self.slots[self._slot] if slot is None else slot)["dev"]
-        cnt = b["count"] if count_on_device else None
+        r = b if rows is None else rows
+        cnt = r["count"] if count_on_device else None
         cp = None if cnt is None else _ptr(cnt)
         per_frame = isinstance(offsets, torch.Tensor) and offsets.dim() == 2
         off = (C.c_float * 6)(*[float(v) for v in (FULL_FRAME if per_frame else offsets)])
         if self.calc_smpl:
-            self.smpl.forward(b["betas"], b["thetas"], cap, cnt, self.settings.root_align, sh["smpl_ws"],
+            self.smpl.forward(r["betas"], r["thetas"], cap, cnt, self.settings.root_align, sh["smpl_ws"],
                               b["verts"], b["joints"], self.stream.cuda_stream)
             if per_frame:
-                _lib.check(lib.b200romp_project_frames(_ptr(b["joints"]), None, _ptr(b["cam"]), cap, cp, _ptr(b["batch_ids"]),
+                _lib.check(lib.b200romp_project_frames(_ptr(b["joints"]), None, _ptr(r["cam"]), cap, cp, _ptr(r["batch_ids"]),
                                                        _ptr(offsets), _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp),
                            "project_frames")
             else:
-                _lib.check(lib.b200romp_project(_ptr(b["joints"]), None, _ptr(b["cam"]), cap, cp, off,
+                _lib.check(lib.b200romp_project(_ptr(b["joints"]), None, _ptr(r["cam"]), cap, cp, off,
                                                 _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp), "project")
         else:   # without SMPL the reference keeps the weak-perspective translation of main.py:166 (no pad info involved)
-            _lib.check(lib.b200romp_project(_ptr(b["cam"]), None, _ptr(b["cam"]), cap, cp, off, None, None,
+            _lib.check(lib.b200romp_project(_ptr(r["cam"]), None, _ptr(r["cam"]), cap, cp, off, None, None,
                                             _ptr(b["cam_trans"]), None, sp), "project")
 
     @torch.no_grad()
@@ -479,7 +487,7 @@ class ROMP(torch.nn.Module):
         chunk i-1 overlap the kernels of chunk i (the two slots of ``forward_batches``).  center_override applies to
         every list, entry k to the k-th image of the list."""
         if self.temporal is not None:
-            raise NotImplementedError("--temporal_optimize smooths one image sequence: call forward() per frame")
+            raise NotImplementedError("--temporal_optimize smooths one image sequence: call forward_video() (or forward() per frame)")
         after_producers(self.stream, self.tdevice, center_override)
 
         def chunks():
@@ -570,6 +578,7 @@ class ROMP(torch.nn.Module):
         """image: HxWx3 uint8 BGR (cv2.imread).  main.py:160-176; preprocessing, model, parse, SMPL and projection all run
         on the GPU - OpenCV is not involved."""
         if self.temporal is not None:
+            self._claim_temporal("forward")
             return self._forward_temporal(image, signal_ID)
         out = self.forward_images([image])[0]
         if out is None:
@@ -628,10 +637,181 @@ class ROMP(torch.nn.Module):
             v["track_ids"] = track_ids                      # main.py:156
         return v
 
+    # ------------------------------------------------------------------------------------------
+    # video mode in batches (-t/--temporal_optimize): the per-frame temporal path of forward, on the batched image path
+    def _claim_temporal(self, user):
+        """forward and forward_video keep separate tracker state: one of them per video (reset_temporal() between)."""
+        if self._temporal_user not in (None, user):
+            raise RuntimeError(f"--temporal_optimize: this instance's video is being run by {self._temporal_user}(); call "
+                               f"reset_temporal() before switching to {user}()")
+        self._temporal_user = user
+
+    def reset_temporal(self):
+        """Start a new video: forget every signal, track id and filter of both forward() and forward_video(); ids count
+        from 1 again."""
+        if self.temporal is None:
+            raise RuntimeError("reset_temporal: this ROMP instance was built without -t/--temporal_optimize")
+        from .temporal import TemporalState
+        sp = C.c_void_p(self.stream.cuda_stream)
+        self.temporal = TemporalState(self.temporal.show_largest, self.temporal.max_signals)
+        _lib.check(self.lib.b200romp_tracks_reset(self._tracks, -1, sp), "tracks_reset")
+        _lib.check(self.lib.b200romp_romp_tracker_reset(self._rtrack, sp), "romp_tracker_reset")
+        self._signal_codes = {}
+        self._temporal_user = None
+
+    def _video_buffers(self, slot):
+        """The track step's outputs of one slot (allocated on first use): the smoothed rows SMPL runs on, the per-row
+        filter slot and track id, the frames' signal codes and pinned read-back mirrors."""
+        if "video" not in slot:
+            dev, cap, B = self.tdevice, self.cap, self.max_batch
+            z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
+            slot["video"] = dict(count=z(1, dtype=torch.int32), batch_ids=z(cap, dtype=torch.int64), thetas=z(cap, 72),
+                                 betas=z(cap, 10), cam=z(cap, 3), slot=z(cap, dtype=torch.int32), track_ids=z(cap, dtype=torch.int32),
+                                 codes=z(B, dtype=torch.int32), codes_host=torch.zeros(B, dtype=torch.int32).pin_memory(),
+                                 codes_h2d=torch.cuda.Event(), counts_host=torch.zeros(2, dtype=torch.int32).pin_memory(), host=None)
+        return slot["video"]
+
+    def run_track_step(self, B, codes, slot):
+        """The video mode's association and One-Euro smoothing of a chunk's B frames (b200romp_romp_track_step), enqueued
+        on self.stream after the parse: no host sync.  ``codes``: the int32 signal code of every frame."""
+        v = self._video_buffers(slot)
+        v["codes_h2d"].synchronize()               # the pinned codes of the slot's previous chunk have been copied
+        v["codes_host"][:B].copy_(torch.as_tensor(codes, dtype=torch.int32))
+        b, s = slot["dev"], self.settings
+        with torch.cuda.stream(self.stream):
+            v["codes"][:B].copy_(v["codes_host"][:B], non_blocking=True)
+            v["codes_h2d"].record(self.stream)
+            _lib.check(self.lib.b200romp_romp_track_step(
+                self._rtrack, B, self.cap, _ptr(b["count"]), _ptr(b["batch_ids"]), _ptr(b["cam"]), _ptr(b["thetas"]),
+                _ptr(b["betas"]), _ptr(v["codes"]), int(self.temporal.show_largest), float(s.smooth_coeff), 30.0, _ptr(v["count"]),
+                _ptr(v["batch_ids"]), _ptr(v["thetas"]), _ptr(v["betas"]), _ptr(v["cam"]), _ptr(v["slot"]), _ptr(v["track_ids"]),
+                C.c_void_p(self.stream.cuda_stream)), "romp_track_step")
+        return v
+
+    def _submit_video(self, imgs, codes, center_override):
+        B = len(imgs)
+        slot, fd = self._preprocess_images(imgs)
+        with torch.cuda.stream(self.stream):
+            self.run_maps(fd)
+            self.run_parse(B, center_override, slot)
+            v = self.run_track_step(B, codes, slot)
+            # tracked: every row (count on the device); --show_largest: the chunk's <= B compacted largest rows
+            self.run_smpl_project(B if self.temporal.show_largest else B * MAX_PERSON, slot["pad"][:B], slot, rows=v)
+            slot["done"].record(self.stream)
+        return slot
+
+    def _read_back_video(self, slot, B, to_numpy):
+        """The chunk's one host sync (both row counts), then its rows -> one result per frame, like forward()."""
+        st, v, d = self.d2h_stream, slot["video"], slot["dev"]
+        st.wait_event(slot["done"])
+        with torch.cuda.stream(st):
+            v["counts_host"][0:1].copy_(d["count"], non_blocking=True)
+            v["counts_host"][1:2].copy_(v["count"], non_blocking=True)
+        st.synchronize()
+        n, m = int(v["counts_host"][0]), int(v["counts_host"][1])
+        res = [None] * B
+        if n == 0:
+            return res
+        tracked = not self.temporal.show_largest
+        per = dict(center_preds=d["center_preds"], center_confs=d["center_confs"], raw=d["thetas"], ids=d["batch_ids"])
+        if tracked:
+            per["track_ids"] = v["track_ids"]
+        rows = dict(cam=v["cam"], smpl_thetas=v["thetas"], smpl_betas=v["betas"], cam_trans=d["cam_trans"], ids=v["batch_ids"])
+        if self.calc_smpl:
+            rows.update(verts=d["verts"], joints=d["joints"], pj2d_org=d["pj2d_org"])
+        if to_numpy:
+            if v["host"] is None:
+                v["host"] = {k: torch.zeros(t.shape, dtype=t.dtype).pin_memory() for k, t in
+                             [("p_" + k, t) for k, t in per.items()] + [("r_" + k, t) for k, t in rows.items()]}
+            h = v["host"]
+            with torch.cuda.stream(st):
+                for k, t in per.items():
+                    h["p_" + k][:n].copy_(t[:n], non_blocking=True)
+                for k, t in rows.items():
+                    h["r_" + k][:m].copy_(t[:m], non_blocking=True)
+            st.synchronize()
+            per = {k: h["p_" + k][:n].numpy() for k in per}
+            rows = {k: h["r_" + k][:m].numpy() for k in rows}
+            own = np.array
+        else:
+            per = {k: t[:n] for k, t in per.items()}
+            rows = {k: t[:m] for k, t in rows.items()}
+            own = lambda t: t.clone()
+        ids = lambda t: t.cpu().numpy() if isinstance(t, torch.Tensor) else t
+        pb = np.searchsorted(ids(per["ids"]), np.arange(B + 1)).tolist()
+        rb = np.searchsorted(ids(rows["ids"]), np.arange(B + 1)).tolist()
+        for i in range(B):
+            s, e, a, z = pb[i], pb[i + 1], rb[i], rb[i + 1]
+            if s == e:
+                continue
+            r = {k: own(rows[k][a:z]) for k in rows if k != "ids"}
+            r.update(global_orient=own(per["raw"][s:e, :3]), body_pose=own(per["raw"][s:e, 3:]),
+                     center_preds=own(per["center_preds"][s:e]), center_confs=own(per["center_confs"][s:e]))
+            if tracked:
+                r["track_ids"] = own(per["track_ids"][s:e])
+            res[i] = r
+        return res
+
+    @torch.no_grad()
+    def forward_video(self, images, signal_IDs=None, to_numpy=True, center_override=None):
+        """Video mode (-t/--temporal_optimize) in batches: ``images`` (HxWx3 uint8 BGR, any sizes, numpy or host / device
+        tensors) are consecutive frames, run in chunks of at most ``max_batch`` through the batched image path, with the
+        association and One-Euro smoothing of every chunk as one kernel between the parse and SMPL (one host sync per
+        chunk).  ``signal_IDs``: one per image (default 0).  Element i of the result is what ``forward(images[i],
+        signal_IDs[i])`` returns in a loop on a fresh instance, or None; nothing is printed.  Like forward's temporal path
+        it keeps the device's closed-form cam_trans (``--cam_trans pnp`` is not applied).  center_override: optional device
+        [n,1,64,64] replacing the images' center maps (tests, measurement)."""
+        sids = None if signal_IDs is None else [signal_IDs]
+        return next(self.forward_video_batches([images], sids, to_numpy, center_override))
+
+    @torch.no_grad()
+    def forward_video_batches(self, batches, signal_IDs=None, to_numpy=True, center_override=None):
+        """Streaming form of ``forward_video`` over an iterable of image lists (consecutive parts of one video; the tracker
+        state carries across lists): yields one result list per input list, in order, on forward_image_batches' two-slot
+        pipeline.  ``signal_IDs``: None (every frame signal 0) or an iterable with one sequence of signal IDs per list.
+        center_override applies to every list, entry k to the k-th image of the list."""
+        if self.temporal is None:
+            raise RuntimeError("forward_video needs -t/--temporal_optimize")
+        after_producers(self.stream, self.tdevice, center_override)
+        sid_iter = None if signal_IDs is None else iter(signal_IDs)
+
+        def chunks():
+            for images in batches:
+                imgs = [image_tensor(x) for x in images]
+                sids = [0] * len(imgs) if sid_iter is None else list(next(sid_iter))
+                if len(sids) != len(imgs):
+                    raise ValueError(f"forward_video: {len(sids)} signal_IDs for {len(imgs)} images")
+                self._claim_temporal("video")
+                codes = [self._signal_codes.setdefault(sid, len(self._signal_codes)) for sid in sids]
+                res = [None] * len(imgs)
+                if not imgs:
+                    yield res, imgs, codes, 0, True
+                for c0 in range(0, len(imgs), self.max_batch):
+                    yield res, imgs[c0:c0 + self.max_batch], codes[c0:c0 + self.max_batch], c0, c0 + self.max_batch >= len(imgs)
+
+        pending = None
+        for res, imgs, codes, c0, last in chunks():
+            co = None if center_override is None else center_override[c0:c0 + len(imgs)]
+            slot = self._submit_video(imgs, codes, co) if imgs else None
+            if pending is not None:
+                done = self._finish_video(*pending, to_numpy)
+                if done is not None:
+                    yield done
+            pending = (slot, res, c0, len(imgs), last)
+        if pending is not None:
+            yield self._finish_video(*pending, to_numpy)
+
+    def _finish_video(self, slot, res, c0, B, last, to_numpy):
+        if slot is not None:
+            res[c0:c0 + B] = self._read_back_video(slot, B, to_numpy)
+        return res if last else None
+
     def __del__(self):
         try:
             if getattr(self, "_tracks", None):
                 self.lib.b200romp_tracks_destroy(self._tracks)
+            if getattr(self, "_rtrack", None):
+                self.lib.b200romp_romp_tracker_destroy(self._rtrack)
         except Exception:
             pass
 
