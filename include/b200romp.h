@@ -190,6 +190,15 @@ int b200romp_project(const float* joints /*[n,71,3]*/, const float* verts /*[n,6
 int b200romp_project_frames(const float* joints, const float* verts, const float* cam, int n, const int* d_count,
                             const long long* batch_ids /*[n]*/, const float* pad_table, float* pj2d_org, float* verts_camed_org,
                             float* cam_trans_weak, float* cam_trans_lsq, b200romp_stream stream);
+/* The reference's default cam_trans (convert_cam_to_3d_trans2 post_parser.py:96-101 -> estimate_translation
+ * utils.py:391-436 -> estimate_translation_cv2 :331-345) with the published EPnP as the solver: joints 0..23 are valid
+ * when their projection pj2d = (xy * s + t + 1) * 256 has y > -2 and z != -2 (:404-419); fewer than 4 valid joints
+ * give (-1,-1,-1) (:420-422); otherwise OpenCV's solvePnPRansac loop (reprojectionError 20, 100 iterations, K =
+ * [[443.4,0,256],[0,443.4,256],[0,0,1]]) around fp64 EPnP, and EPnP on the best inlier set; no model -> (-1,-1,-1).
+ * Overwrites cam_trans [n,3] for the first min(n, *d_count) persons (all n when d_count is NULL).  inlier_mask (may be
+ * NULL): per person, bit i = the i-th valid joint (in joint order) is an inlier of the returned pose.  Stream-ordered. */
+int b200romp_cam_trans_pnp(const float* joints /*[n,71,3]*/, const float* cam /*[n,3]*/, int n, const int* d_count,
+                           float* cam_trans /*[n,3]*/, int* inlier_mask /*[n] or NULL*/, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
  * BEV variant (simple_romp/bev): the stages of BEVv1.forward (bev/model.py:232-250) and of

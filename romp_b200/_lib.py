@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "lib", "libb200romp.so")
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "romp_track.cu", "resnet_ops.cu"]
+SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "pnp.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "romp_track.cu", "resnet_ops.cu"]
 
 F32, BF16, U8 = 0, 1, 2
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_WGMMA, ENGINE_TF32 = 0, 1, 2, 3
@@ -146,6 +146,7 @@ def load():
     _sig(lib.b200romp_smpl_forward, i32, vp, vp, i32, vp, i32, vp, i32, vp, vp, vp, vp)
     _sig(lib.b200romp_project, i32, vp, vp, vp, i32, vp, fp, vp, vp, vp, vp, vp)
     _sig(lib.b200romp_project_frames, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp)
+    _sig(lib.b200romp_cam_trans_pnp, i32, vp, vp, i32, vp, vp, vp, vp)
     _sig(lib.b200romp_bev_create, vp, i32, C.POINTER(BevWeights))
     _sig(lib.b200romp_bev_destroy, None, vp)
     _sig(lib.b200romp_bev_bv_input, i32, vp, vp, i32, i32, i32, vp, i32, vp)
@@ -196,6 +197,7 @@ EXPORTS = [
     "b200romp_conv2d",
     "b200romp_parse", "b200romp_parse_workspace_bytes", "b200romp_smpl_create", "b200romp_smpl_destroy",
     "b200romp_smpl_workspace_floats", "b200romp_smpl_forward", "b200romp_project", "b200romp_project_frames",
+    "b200romp_cam_trans_pnp",
     "b200romp_bev_create", "b200romp_bev_destroy", "b200romp_bev_bv_input", "b200romp_bev_center3d",
     "b200romp_bev_parse_workspace_bytes", "b200romp_bev_parse3d", "b200romp_bev_regress", "b200romp_bev_post",
     "b200romp_bev_post_frames", "b200romp_bev_crop_post", "b200romp_bev_long_merge_workspace_bytes", "b200romp_bev_long_merge",

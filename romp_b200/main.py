@@ -60,9 +60,11 @@ def romp_settings(input_args=sys.argv[1:]):
     parser.add_argument("--backbone", type=str, default="hrnet32", choices=["hrnet32", "resnet50"],
                         help="hrnet32 = simple_romp's ROMPv1 (model.py); resnet50 = the training package's ResNet-50 variant "
                              "(romp/lib/models/resnet_50.py; workload cfg1), state dict with the same head keys")
-    parser.add_argument("--cam_trans", type=str, default="lsq", choices=["lsq", "pnp"],
+    parser.add_argument("--cam_trans", type=str, default="lsq", choices=["lsq", "pnp", "epnp"],
                         help="cam_trans estimator: lsq = closed-form least squares on the GPU (the reference's fallback, "
-                             "utils.py:347-389); pnp = the reference's default cv2.solvePnPRansac per person on the host")
+                             "utils.py:347-389); pnp = the reference's default cv2.solvePnPRansac per person on the host; "
+                             "epnp = the reference's RANSAC loop and validity mask on the GPU, with the published EPnP as "
+                             "its solver (every entry point)")
     args = parser.parse_args(input_args)
     if not os.path.exists(args.smpl_path):
         alt = args.smpl_path.replace("SMPL_NEUTRAL.pth", "smpl_packed_info.pth")   # main.py:50-52
@@ -337,6 +339,9 @@ class ROMP(torch.nn.Module):
             else:
                 _lib.check(lib.b200romp_project(_ptr(b["joints"]), None, _ptr(r["cam"]), cap, cp, off,
                                                 _ptr(b["pj2d_org"]), None, None, _ptr(b["cam_trans"]), sp), "project")
+            if getattr(self.settings, "cam_trans", "lsq") == "epnp":    # overwrites the closed form in place
+                _lib.check(lib.b200romp_cam_trans_pnp(_ptr(b["joints"]), _ptr(r["cam"]), cap, cp, _ptr(b["cam_trans"]), None, sp),
+                           "cam_trans_pnp")
         else:   # without SMPL the reference keeps the weak-perspective translation of main.py:166 (no pad info involved)
             _lib.check(lib.b200romp_project(_ptr(r["cam"]), None, _ptr(r["cam"]), cap, cp, off, None, None,
                                             _ptr(b["cam_trans"]), None, sp), "project")
@@ -759,7 +764,8 @@ class ROMP(torch.nn.Module):
         association and One-Euro smoothing of every chunk as one kernel between the parse and SMPL (one host sync per
         chunk).  ``signal_IDs``: one per image (default 0).  Element i of the result is what ``forward(images[i],
         signal_IDs[i])`` returns in a loop on a fresh instance, or None; nothing is printed.  Like forward's temporal path
-        it keeps the device's closed-form cam_trans (``--cam_trans pnp`` is not applied).  center_override: optional device
+        it keeps the device's cam_trans: the closed form, or ``--cam_trans epnp`` on the smoothed rows (``--cam_trans pnp``,
+        a host step, is not applied).  center_override: optional device
         [n,1,64,64] replacing the images' center maps (tests, measurement)."""
         sids = None if signal_IDs is None else [signal_IDs]
         return next(self.forward_video_batches([images], sids, to_numpy, center_override))
