@@ -5,7 +5,8 @@ True and therefore overrides the thresholds with ``long_conf_dict``), ``BEV(sett
 mirrors bev/main.py:91-258: normal images run as one 512x512 frame, and in crowd mode images at least twice as wide as
 high run through ``process_long_image`` (the reference's overlapping crops, batched through the model, with the per-crop
 and merged filters on the device).  ``forward_batch`` is the batched entry point for normal frames, ``forward_images`` the
-batched ``forward`` on raw images of different sizes (each frame with its own geometry).
+batched ``forward`` on raw images of different sizes (each frame with its own geometry); ``forward_batches`` and
+``forward_image_batches`` stream them on two slots, staging and reading back neighbouring chunks while a chunk's kernels run.
 Per-frame semantics of the two post filters (bev/post_parser.py:167-222) are preserved by applying them per
 ``pred_batch_ids`` group on the device.  Python only allocates buffers and sequences library calls.
 """
@@ -23,7 +24,7 @@ import torch
 from . import _lib, graph
 from ._lib import BF16, F32, U8
 from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
-from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, split_by_frame
+from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
 long_conf_dict = {1: [0.12, 20, 1.5, 0.46], 2: [0.08, 20, 1.6, 0.8]}
@@ -31,6 +32,7 @@ model_dict = {1: "BEV_ft_agora.pth", 2: "BEV.pth"}
 N_PARAMS = 146                                                       # 3 cam + 22*6 + 11 betas, bev/model.py:116
 TRACKER_MAX_TRACKS = 128                                             # live tracks (tracked + lost) of the video mode
 MAX_SIGNALS = 4                                                      # filter sets of the video mode, the oldest evicted
+LARGEST_KEYS = ("params_pred", "center_confs", "pred_batch_ids")     # --show_largest: one row per detection, not per output
 
 
 def bev_settings(input_args=sys.argv[1:]):
@@ -137,7 +139,6 @@ class BEV(torch.nn.Module):
         self.tdevice = torch.device("cuda", self.device_index)
         torch.cuda.set_device(self.tdevice)
         self.precision = getattr(s, "precision", "bf16")
-        self._frames = {}                              # frame buffers by (dtype, B)
         self.max_batch = B = int(getattr(s, "max_batch", 32))
         if state_dict is None:
             state_dict = torch.load(s.model_path, map_location="cpu")          # bev/main.py:101 (strict=False)
@@ -176,30 +177,56 @@ class BEV(torch.nn.Module):
         self.act_code = BF16 if self.precision == "bf16" else F32
         z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
         i64, i32 = torch.int64, torch.int32
-        self.buf = dict(
+        # shared scratch: only touched by kernels on self.stream, in order
+        self.shared = dict(
             maps_fv=z(B, 4, 128, 128), fv_feats=z(B, 128, 128, 128, dtype=act), img_feats=z(B, 128, 128, graph.bev_feats_channels(self.precision), dtype=act),
             bv_in=z(B, 1, 128, 2560, dtype=act), bv_out=z(B, 1, 128, 128, dtype=act),
             c3d_tmp=z(B, 64, 128, 128), center3d=z(B, 64, 128, 128),
             parse_ws=torch.zeros(int(self.lib.b200romp_bev_parse_workspace_bytes(B)), dtype=torch.uint8, device=dev),
-            count=z(1, dtype=i32), batch_ids=z(cap, dtype=i64), czyx=z(cap, 3, dtype=i64), conf=z(cap),
-            params_pred=z(cap, N_PARAMS), cam_czyx=z(cap, 3, dtype=i64), cam=z(cap, 3), thetas=z(cap, 72), betas=z(cap, 11),
-            cam_trans=z(cap, 3), pj2d_org=z(cap, 71, 2), keep=z(cap, dtype=i32), sel=z(cap, dtype=i32), count2=z(1, dtype=i32),
-        )
+            czyx=z(cap, 3, dtype=i64), cam_czyx=z(cap, 3, dtype=i64), pj2d_org=z(cap, 71, 2), keep=z(cap, dtype=i32), sel=z(cap, dtype=i32))
         if self.calc_smpl:
-            self.buf.update(verts=z(cap, 6890, 3), joints=z(cap, 71, 3), verts_smil=z(cap, 6890, 3), joints_smil=z(cap, 71, 3),
-                            smpl_ws=z(cap, self.smpla.ws_floats))
-        # compacted outputs (after the per-frame post filters)
-        self.out = {k: torch.zeros_like(self.buf[k]) for k in ("batch_ids", "conf", "params_pred", "cam", "thetas", "betas",
-                                                               "cam_trans", "pj2d_org")}
-        if self.calc_smpl:
-            self.out.update(verts=torch.zeros_like(self.buf["verts"]), joints=torch.zeros_like(self.buf["joints"]))
-        self.count_host = torch.zeros(2, dtype=torch.int32).pin_memory()
-        self.pad_table = z(B, 6)                       # per-frame pad info of forward_images / forward_batch([B,6] offsets)
-        self.raw = RawStager(dev)                       # raw image staging of forward_images
+            self.shared.update(verts=z(cap, 6890, 3), joints=z(cap, 71, 3), verts_smil=z(cap, 6890, 3), joints_smil=z(cap, 71, 3),
+                               smpl_ws=z(cap, self.smpla.ws_floats))
+        # two slots of what a result reads (the regressor's rows, the compacted rows after the per-frame post filters), with
+        # their frames, staging and events, so that chunk i+1 is staged and chunk i-1 read back while chunk i's kernels run
+        self.slots = []
+        for _ in range(2):
+            d = dict(count=z(1, dtype=i32), batch_ids=z(cap, dtype=i64), conf=z(cap), params_pred=z(cap, N_PARAMS), cam=z(cap, 3),
+                     thetas=z(cap, 72), betas=z(cap, 11), cam_trans=z(cap, 3), count2=z(1, dtype=i32))
+            rows = {**self.shared, **d}
+            keys = ("batch_ids", "conf", "params_pred", "cam", "thetas", "betas", "cam_trans", "pj2d_org") + (("verts", "joints") if self.calc_smpl else ())
+            # -t reads the tracker's compacted rows (tout): one set of these serves both slots, for direct run_post calls
+            out = self.slots[0]["out"] if self.temporal and self.slots else {k: torch.zeros_like(rows[k]) for k in keys}
+            self.slots.append(dict(dev=d, out=out, frames={}, pad=z(B, 6), raw=RawStager(dev), done=torch.cuda.Event(),
+                                   h2d=torch.cuda.Event(), counts_host=torch.zeros(6 + B, dtype=i32).pin_memory(), host={}))
+        self._slot = 0
+        self.copy_stream = torch.cuda.Stream(device=dev)
+        self.d2h_stream = torch.cuda.Stream(device=dev)
+        self.count_host = torch.zeros(2, dtype=torch.int32).pin_memory()      # the long-image mode's read-back
+
+    @property
+    def buf(self):
+        """device buffers of the slot used by the most recent chunk (+ the shared scratch)"""
+        return {**self.shared, **self.slots[self._slot]["dev"]}
+
+    @property
+    def out(self):
+        """compacted rows (after the per-frame post filters) of the slot used by the most recent chunk"""
+        return self.slots[self._slot]["out"]
+
+    @property
+    def tbuf(self):
+        """-t: the track step's rows of the slot used by the most recent chunk (+ the shared scratch)"""
+        return {**self.tshared, **self.slots[self._slot]["tdev"]}
+
+    @property
+    def tout(self):
+        """-t: the compacted rows of the slot used by the most recent chunk"""
+        return self.slots[self._slot]["tout"]
 
     def _alloc_temporal(self, B):
         """The video mode (bev/main.py:109-121,260-287): one tracker per instance (shared by every signal_ID), the
-        filter sets of MAX_SIGNALS signals, and row buffers for up to 2 x 64 rows per frame."""
+        filter sets of MAX_SIGNALS signals, and per slot row buffers for up to 2 x 64 rows per frame."""
         dev, R = self.tdevice, 2 * B * MAX_PERSON
         self.trk = self.lib.b200romp_bev_tracker_create(self.device_index, TRACKER_MAX_TRACKS, MAX_SIGNALS)
         if not self.trk:
@@ -207,21 +234,21 @@ class BEV(torch.nn.Module):
         self.signals = {}                              # signal_ID -> filter set, oldest first (ROMP's TemporalState)
         z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
         i64, i32 = torch.int64, torch.int32
-        self.tbuf = dict(count=z(1, dtype=i32), batch_ids=z(R, dtype=i64), track_ids=z(R, dtype=i32), det=z(R, dtype=i32),
-                         thetas=z(R, 72), betas=z(R, 11), cam=z(R, 3), cam_trans=z(R, 3), params_pred=z(R, N_PARAMS), conf=z(R),
-                         status=z(2 + B, dtype=i32), sig=z(B, dtype=i32), pj2d_org=z(R, 71, 2), keep=z(R, dtype=i32),
-                         sel=z(R, dtype=i32), count2=z(1, dtype=i32))
+        self.tshared = dict(det=z(R, dtype=i32), pj2d_org=z(R, 71, 2), keep=z(R, dtype=i32), sel=z(R, dtype=i32))
         if self.calc_smpl:
-            self.tbuf.update(verts=z(R, 6890, 3), joints=z(R, 71, 3), verts_smil=z(R, 6890, 3), joints_smil=z(R, 71, 3),
-                             smpl_ws=z(R, self.smpla.ws_floats))
-        self.tout = {k: torch.zeros_like(self.tbuf[k]) for k in ("batch_ids", "track_ids", "conf", "params_pred", "cam", "thetas",
-                                                                "betas", "cam_trans", "pj2d_org")}
-        if self.calc_smpl:
-            self.tout.update(verts=torch.zeros_like(self.tbuf["verts"]), joints=torch.zeros_like(self.tbuf["joints"]))
-        # the batch's one read-back: detected, rows, kept rows, then the kernel's status, frame_id and rows per frame
-        self.tsync_host = torch.zeros(5 + B, dtype=torch.int32).pin_memory()
+            self.tshared.update(verts=z(R, 6890, 3), joints=z(R, 71, 3), verts_smil=z(R, 6890, 3), joints_smil=z(R, 71, 3),
+                                smpl_ws=z(R, self.smpla.ws_floats))
+        for slot in self.slots:
+            # status: the kernel's status, frame_id and rows per frame
+            t = dict(count=z(1, dtype=i32), batch_ids=z(R, dtype=i64), track_ids=z(R, dtype=i32), thetas=z(R, 72), betas=z(R, 11),
+                     cam=z(R, 3), cam_trans=z(R, 3), params_pred=z(R, N_PARAMS), conf=z(R), status=z(2 + B, dtype=i32),
+                     sig=z(B, dtype=i32), count2=z(1, dtype=i32))
+            rows = {**self.tshared, **t}
+            keys = ("batch_ids", "track_ids", "conf", "params_pred", "cam", "thetas", "betas", "cam_trans", "pj2d_org") + \
+                (("verts", "joints") if self.calc_smpl else ())
+            slot.update(tdev=t, tout={k: torch.zeros_like(rows[k]) for k in keys}, sig_host=torch.zeros(B, dtype=i32).pin_memory(),
+                        sig_h2d=torch.cuda.Event())
         self.frame_id = 0                              # tracker frames so far (frames with a detection)
-        self.tsig_host = torch.zeros(B, dtype=torch.int32).pin_memory()
 
     def _signal_slots(self, signal_IDs):
         """filter set of every frame's signal_ID; a new signal beyond MAX_SIGNALS evicts the oldest one (its filters are
@@ -253,10 +280,12 @@ class BEV(torch.nn.Module):
     def run_temporal(self, B, signal_IDs):
         """BEV.temporal_optimization (bev/main.py:165-169,260-287) of the batch's frames in order: one kernel
         (b200romp_bev_track_step) between the regressor and SMPL-A, writing the smoothed rows to ``self.tbuf``."""
-        b, t = self.buf, self.tbuf
+        b, t, slot = self.buf, self.tbuf, self.slots[self._slot]
         slots = self._signal_slots(signal_IDs)
-        self.tsig_host[:B].copy_(torch.tensor(slots, dtype=torch.int32))
-        t["sig"][:B].copy_(self.tsig_host[:B], non_blocking=True)
+        slot["sig_h2d"].synchronize()                 # the slot's previous chunk has copied its signal slots
+        slot["sig_host"][:B].copy_(torch.tensor(slots, dtype=torch.int32))
+        t["sig"][:B].copy_(slot["sig_host"][:B], non_blocking=True)
+        slot["sig_h2d"].record(self.stream)
         R = 2 * B * MAX_PERSON
         _lib.check(self.lib.b200romp_bev_track_step(
             self.trk, B, B * MAX_PERSON, _ptr(b["count"]), _ptr(b["batch_ids"]), _ptr(b["conf"]), _ptr(b["cam"]), _ptr(b["cam_trans"]),
@@ -269,52 +298,6 @@ class BEV(torch.nn.Module):
     def run_post_temporal(self, B, offsets, img_max_side=512.0):
         """run_post on the tracker's rows (up to 2 x 64 per frame)."""
         self.run_post(B, offsets, img_max_side, self.tbuf, self.tout, 2 * B * MAX_PERSON, self.tbuf["count"])
-
-    def _collect_temporal(self, B, to_numpy):
-        """(batch result dict, rows per frame) after the host sync; raises on a full track table."""
-        h, t = self.tsync_host, self.tbuf
-        with torch.cuda.stream(self.stream):
-            h[0:1].copy_(self.buf["count"], non_blocking=True)
-            h[1:2].copy_(t["count"], non_blocking=True)
-            h[2:3].copy_(t["count2"], non_blocking=True)
-            h[3:5 + B].copy_(t["status"][:2 + B], non_blocking=True)
-        self.stream.synchronize()
-        n_det, n_rows, n_kept, status = int(h[0]), int(h[1]), int(h[2]), int(h[3])
-        self.frame_id = int(h[4])
-        if status:
-            raise RuntimeError("BEV video mode: " + (f"more than {TRACKER_MAX_TRACKS} live tracks" if status == 1 else "too many rows")
-                               + "; call reset_temporal() before the next frame")
-        src, n = (self.tout, n_kept) if self.calc_smpl else (self.tbuf, n_rows)
-        bid = src["batch_ids"][:n]
-        out = self._result(src, n, bid, False)
-        out["_bid"] = bid
-        if not self.show_largest:
-            out["track_ids"] = src["track_ids"][:n]
-        else:                                           # bev/main.py:262-267: only thetas / betas / cam are cut to one row
-            out.update(params_pred=self.buf["params_pred"][:n_det], center_confs=self.buf["conf"][:n_det],
-                       pred_batch_ids=self.buf["batch_ids"][:n_det])
-        rows = {b for b in range(B) if int(h[5 + b])}                # frames the tracker gave rows (before the filters)
-        if to_numpy:
-            with torch.cuda.stream(self.stream):
-                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
-        return out, rows
-
-    def _split_temporal(self, out, B, rows, to_numpy):
-        """per-frame dicts of a temporal batch result (None for a frame without rows), pred_batch_ids set to 0."""
-        res = []
-        for b in range(B):
-            if b not in rows:
-                res.append(None)
-                continue
-            r = {}
-            for k, v in out.items():
-                ids = out["pred_batch_ids"] if (self.show_largest and k in ("params_pred", "center_confs", "pred_batch_ids")) else out["_bid"]
-                r[k] = v[ids == b]
-            n = len(r["pred_batch_ids"])
-            r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
-            r.pop("_bid")
-            res.append(r)
-        return res
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -380,56 +363,180 @@ class BEV(torch.nn.Module):
             _lib.check(lib.b200romp_gather_rows(_ptr(src), row, _ptr(b["sel"]), _ptr(b["count2"]), cap, _ptr(dst), sp), "gather_rows")
 
     def _counts(self, detected, kept):
-        """The host sync of a result: (persons detected, persons kept by the filters) from two device counters."""
+        """The host sync of a long-image result: (persons detected, persons kept by the filters) from two device counters."""
         with torch.cuda.stream(self.stream):
             self.count_host[0:1].copy_(detected, non_blocking=True)
             self.count_host[1:2].copy_(kept, non_blocking=True)
         self.stream.synchronize()
         return int(self.count_host[0]), int(self.count_host[1])
 
-    def _result(self, src, n, batch_ids, to_numpy):
-        """The output dict (result_keys, plus the SMPL outputs) from the first n rows of the buffers ``src``."""
+    def _result(self, src, n, batch_ids):
+        """The output dict (result_keys, plus the SMPL outputs): device views of the first n rows of the buffers ``src``."""
         out = {"smpl_thetas": src["thetas"][:n], "smpl_betas": src["betas"][:n], "cam": src["cam"][:n], "cam_trans": src["cam_trans"][:n],
                "params_pred": src["params_pred"][:n], "center_confs": src["conf"][:n], "pred_batch_ids": batch_ids}
         if self.calc_smpl:
             out.update(verts=src["verts"][:n], joints=src["joints"][:n], pj2d_org=src["pj2d_org"][:n])
-        if to_numpy:
-            with torch.cuda.stream(self.stream):
-                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
         return out
 
-    def collect(self, to_numpy=True):
-        n_det, n = self._counts(self.buf["count"], self.buf["count2"])
-        if n_det == 0:
+    def _read_back(self, slot, B, to_numpy, temporal, split=False):
+        """A chunk's result, on the read-back stream after the slot's kernels: one sync for its row counts (and with
+        ``temporal`` the tracker's status), then one more for its valid rows and their frame ids.  Returns None when the
+        chunk has no result (nobody detected; with -t no tracker rows), else (out, rows, det, frames): the batch result
+        (numpy arrays, views of the slot's pinned mirrors with ``split``, or device views without to_numpy), the frame of
+        each of its rows and of each detection (host int64), and the frames that have a result.  Raises on a nonzero
+        tracker status."""
+        st, d, h = self.d2h_stream, slot["dev"], slot["counts_host"]
+        st.wait_event(slot["done"])
+        with torch.cuda.stream(st):
+            h[0:1].copy_(d["count"], non_blocking=True)
+            h[1:2].copy_(d["count2"], non_blocking=True)
+            if temporal:
+                t = slot["tdev"]
+                h[2:3].copy_(t["count"], non_blocking=True)
+                h[3:4].copy_(t["count2"], non_blocking=True)
+                h[4:6 + B].copy_(t["status"][:2 + B], non_blocking=True)
+        st.synchronize()
+        n_det, frames = int(h[0]), None
+        if temporal:
+            n_rows, n_kept, status = int(h[2]), int(h[3]), int(h[4])
+            self.frame_id = int(h[5])
+            if status:
+                raise RuntimeError("BEV video mode: " + (f"more than {TRACKER_MAX_TRACKS} live tracks" if status == 1 else "too many rows")
+                                   + "; call reset_temporal() before the next frame")
+            frames = [b for b in range(B) if int(h[6 + b])]              # frames the tracker gave rows (before the filters)
+            if not frames:
+                return None
+            src, n = (slot["tout"], n_kept) if self.calc_smpl else (t, n_rows)
+        elif n_det == 0:
             return None
-        src, n = (self.out, n) if self.calc_smpl else (self.buf, n_det)
-        return self._result(src, n, src["batch_ids"][:n], to_numpy)
+        else:
+            src, n = (slot["out"], int(h[1])) if self.calc_smpl else (d, n_det)
+        out = self._result(src, n, src["batch_ids"][:n])
+        if temporal and self.show_largest:           # bev/main.py:262-267: only thetas / betas / cam are cut to one row
+            out.update(params_pred=d["params_pred"][:n_det], center_confs=d["conf"][:n_det], pred_batch_ids=d["batch_ids"][:n_det])
+        elif temporal:
+            out["track_ids"] = src["track_ids"][:n]
+        ids = dict(_rows=src["batch_ids"][:n], _det=d["batch_ids"][:n_det])
+        # a result split per frame is copied out of pinned mirrors frame by frame; a whole-batch result goes straight
+        # into arrays of its own (a mirror would cost it a second host copy)
+        fetch = {**ids, **out} if to_numpy and split else ids
+        host = slot["host"]
+        with torch.cuda.stream(st):
+            for k, v in fetch.items():
+                if k not in host or len(host[k]) < len(v):      # pinned mirrors, allocated on first use, grown on demand
+                    rows = max(len(v), 2 * len(host.get(k, ())), 64)
+                    host[k] = torch.empty((rows, *v.shape[1:]), dtype=v.dtype, pin_memory=True)
+                host[k][:len(v)].copy_(v, non_blocking=True)
+            if to_numpy and not split:
+                out = {k: v.cpu().numpy() for k, v in out.items()}
+        st.synchronize()
+        got = {k: host[k][:len(v)].numpy() for k, v in fetch.items()}
+        if to_numpy and split:
+            out = {k: got[k] for k in out}
+        if frames is None:
+            frames = np.unique(got["_det"]).tolist()
+        return out, got["_rows"], got["_det"], frames
 
-    @torch.no_grad()
-    def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0, signal_IDs=None):
-        """frames [B,512,512,3] padded+resized like img_preprocess.  ``offsets``: one pad info [top,bottom,left,right,h,w]
-        for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
-        suppressing with its own max(h, w) (``img_max_side`` is not used).  With -t the frames are consecutive video
-        frames, tracked and smoothed in order (``signal_IDs``: one per frame, default 0); the result adds ``track_ids``."""
-        if isinstance(frames, np.ndarray):
-            frames = torch.from_numpy(frames)
-        B = frames.shape[0]
-        after_producers(self.stream, self.tdevice, frames, center3d_override, offsets)
-        fd = frame_buffer(self._frames, frames.dtype, B, self.tdevice)
-        with torch.cuda.stream(self.stream):
-            fd.copy_(frames, non_blocking=True)
-            offsets = frame_offsets(offsets, self.pad_table, B)
+    @staticmethod
+    def _batch(got):
+        """forward_batch's dict from a read-back: host arrays, or device views"""
+        return None if got is None else got[0]
+
+    def _per_frame(self, got, B, to_numpy):
+        """forward_images' per-frame dicts from a chunk's read-back: None for a frame without a result, else the frame's
+        rows of every key (arrays that own their memory, or device copies) with pred_batch_ids zeroed.  The rows come in
+        frame order, so each frame's rows are one host searchsorted on their frame ids."""
+        res = [None] * B
+        if got is None:
+            return res
+        out, rows, det, frames = got
+        br = np.searchsorted(rows, np.arange(B + 1)).tolist()
+        bd = np.searchsorted(det, np.arange(B + 1)).tolist()
+        largest = LARGEST_KEYS if self.temporal and self.show_largest else ()
+        with torch.cuda.stream(self.d2h_stream):
+            for f in frames:
+                r = {}
+                for k, v in out.items():
+                    s, e = (bd[f], bd[f + 1]) if k in largest else (br[f], br[f + 1])
+                    r[k] = np.array(v[s:e]) if to_numpy else v[s:e].clone()
+                n = len(r["pred_batch_ids"])
+                r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
+                res[f] = r
+        if not to_numpy:
+            self.d2h_stream.synchronize()           # the copies have read the slot before its next chunk overwrites it
+        return res
+
+    def collect(self, to_numpy=True):
+        """The result of the frames that run_model / run_post last enqueued on self.stream (the current slot, without the
+        video mode's tracker rows): one dict with pred_batch_ids, or None when nobody was detected."""
+        slot = self.slots[self._slot]
+        slot["done"].record(self.stream)
+        return self._batch(self._read_back(slot, 0, to_numpy, False))
+
+    def _next_slot(self):
+        self._slot ^= 1
+        return self.slots[self._slot]
+
+    def _run(self, slot, fd, B, offsets, img_max_side, center3d_override, signal_IDs):
+        """A chunk's kernels on self.stream after its frames fd: model, with -t the track step, post filters; then the
+        slot's done event (also when a chunk is refused on the way: the slot is free after what was enqueued)."""
+        try:
             self.run_model(fd, center3d_override)
             if self.temporal:
                 self.run_temporal(B, [0] * B if signal_IDs is None else list(signal_IDs))
                 self.run_post_temporal(B, offsets, img_max_side)
             else:
                 self.run_post(B, offsets, img_max_side)
-        if self.temporal:
-            out, rows = self._collect_temporal(B, to_numpy)
-            out.pop("_bid")
-            return out if rows else None
-        return self.collect(to_numpy)
+        finally:
+            slot["done"].record(self.stream)
+
+    @torch.no_grad()
+    def forward_batch(self, frames, offsets=None, to_numpy=True, center3d_override=None, img_max_side=512.0, signal_IDs=None):
+        """frames [B,512,512,3] padded+resized like img_preprocess.  ``offsets``: one pad info [top,bottom,left,right,h,w]
+        for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
+        suppressing with its own max(h, w) (``img_max_side`` is not used).  With -t the frames are consecutive video
+        frames, tracked and smoothed in order (``signal_IDs``: one per frame, default 0); the result adds ``track_ids``.
+        ``to_numpy=False`` returns device views of the slot's rows, valid until the second-next batch."""
+        sids = None if signal_IDs is None else [signal_IDs]
+        return next(self.forward_batches([frames], offsets, center3d_override, to_numpy, img_max_side, sids))
+
+    @torch.no_grad()
+    def forward_batches(self, batches, offsets=None, center3d_override=None, to_numpy=True, img_max_side=512.0, signal_IDs=None):
+        """Streaming form of ``forward_batch`` over an iterable of frame batches [B,512,512,3] (a video): yields what
+        ``forward_batch`` returns for each batch, in order.  Each batch goes into the next of two slots: its frames are
+        copied into the slot's frame buffer on the copy stream, so the copy of batch i+1 and the read-back of batch i-1
+        overlap the kernels of batch i.  The generator goes on once a host batch has been copied, so a caller may refill
+        one pinned buffer between batches.  ``offsets``, ``center3d_override`` and ``img_max_side`` apply to every batch;
+        with -t the batches are consecutive parts of one video and ``signal_IDs`` is None or one sequence per batch."""
+        after_producers(self.stream, self.tdevice, center3d_override, offsets)
+        sid_iter = None if signal_IDs is None else iter(signal_IDs)
+        pending = None
+        for frames in batches:
+            slot = self._submit_frames(frames, offsets, center3d_override, img_max_side, None if sid_iter is None else next(sid_iter))
+            if pending is not None:
+                yield self._batch(self._read_back(*pending, to_numpy, self.temporal))
+            pending = slot
+        if pending is not None:
+            yield self._batch(self._read_back(*pending, to_numpy, self.temporal))
+
+    def _submit_frames(self, frames, offsets, center3d_override, img_max_side, signal_IDs):
+        """One batch of frames into the next slot; returns (slot, B) once host frames have been copied."""
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(frames)
+        B = frames.shape[0]
+        slot = self._next_slot()
+        fd = frame_buffer(slot["frames"], frames.dtype, B, self.tdevice)
+        after_producers(self.copy_stream, self.tdevice, frames)
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_event(slot["done"])          # the slot's previous kernels no longer read fd
+            fd.copy_(frames, non_blocking=True)
+            slot["h2d"].record(self.copy_stream)
+        with torch.cuda.stream(self.stream):
+            self.stream.wait_event(slot["h2d"])
+            self._run(slot, fd, B, frame_offsets(offsets, slot["pad"], B), img_max_side, center3d_override, signal_IDs)
+        if not frames.is_cuda:
+            slot["h2d"].synchronize()
+        return slot, B
 
     @torch.no_grad()
     def forward_images(self, images, to_numpy=True, center3d_override=None, signal_IDs=None):
@@ -438,61 +545,96 @@ class BEV(torch.nn.Module):
         Normal images run in chunks of at most ``max_batch`` through one preprocessing kernel per chunk (the GPU kernel,
         not the host OpenCV resize of ``forward``) and b200romp_bev_post_frames, each frame with its own pad info and
         suppression threshold; element i then equals ``forward_batch`` on image i's GPU-preprocessed frame with its pad
-        info and ``img_max_side = max(h, w)``.  In crowd mode images with w/h >= 2 go one by one through
-        ``process_long_image``.  center3d_override: optional device [n_normal,64,128,128] for the normal images in order.
+        info and ``img_max_side = max(h, w)``.  A frame with a detection whose persons were all filtered out gives a dict
+        of empty arrays.  In crowd mode images with w/h >= 2 go one by one through ``process_long_image``.
+        center3d_override: optional device [n_normal,64,128,128] for the normal images in order.
         With -t the normal images are consecutive video frames (``signal_IDs``: one per image, default 0), tracked and
         smoothed in list order; wide crowd-mode images are neither tracked nor smoothed (bev/main.py:140-143)."""
-        imgs = [image_tensor(x) for x in images]
-        res = [None] * len(imgs)
-        normal = []
-        for i, t in enumerate(imgs):
-            if self.settings.crowd and t.shape[1] / t.shape[0] >= 2:
-                if getattr(self.settings, "show_patch_results", False):
-                    raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
-                res[i] = self.process_long_image(t, to_numpy=to_numpy)
-            else:
-                normal.append(i)
-        if center3d_override is not None:
-            assert center3d_override.is_cuda and center3d_override.shape[0] == len(normal)
-            after_producers(self.stream, self.tdevice, center3d_override)
-        for c0 in range(0, len(normal), self.max_batch):
-            idx = normal[c0:c0 + self.max_batch]
-            sigs = [0 if signal_IDs is None else signal_IDs[i] for i in idx]
-            for i, r in zip(idx, self._forward_chunk([imgs[i] for i in idx], to_numpy,
-                                                     None if center3d_override is None else center3d_override[c0:c0 + len(idx)], sigs)):
-                res[i] = r
-        return res
+        sids = None if signal_IDs is None else [signal_IDs]
+        return next(self.forward_image_batches([images], to_numpy, center3d_override, sids))
 
-    def _forward_chunk(self, imgs, to_numpy, center3d_override, signal_IDs=None):
-        """One chunk of normal images: staging + one H2D, batched preprocessing, model, per-frame post; one host sync."""
+    @torch.no_grad()
+    def forward_image_batches(self, batches, to_numpy=True, center3d_override=None, signal_IDs=None):
+        """Streaming form of ``forward_images`` over an iterable of image lists: yields, for each list, what
+        ``forward_images`` returns for it, in order.  Each chunk of at most ``max_batch`` normal images is staged into
+        its slot's pinned buffer and sent with one H2D on the copy stream (device images are read in place), so staging
+        chunk i+1 and reading back chunk i-1 overlap the kernels of chunk i (the two slots of ``forward_batches``).  A
+        wide crowd-mode image drains the pipeline and runs through ``process_long_image`` between its list's chunks.
+        center3d_override applies to every list, entry k to the k-th normal image of the list.  With -t the lists are
+        consecutive parts of one video (tracker and filters carry across them) and ``signal_IDs`` is None or one sequence
+        per list."""
+        if center3d_override is not None:
+            assert center3d_override.is_cuda
+        after_producers(self.stream, self.tdevice, center3d_override)
+        sid_iter = None if signal_IDs is None else iter(signal_IDs)
+
+        def chunks():
+            """(images, signal IDs, result list, the chunk's normal images, their 3-D centre maps, the wide images to run
+            before the chunk, last chunk of the list)"""
+            for images in batches:
+                imgs = [image_tensor(x) for x in images]
+                sids = [0] * len(imgs) if sid_iter is None else list(next(sid_iter))
+                if len(sids) != len(imgs):
+                    raise ValueError(f"forward_image_batches: {len(sids)} signal_IDs for {len(imgs)} images")
+                wide = [i for i, t in enumerate(imgs) if self.settings.crowd and t.shape[1] / t.shape[0] >= 2]
+                normal = [i for i in range(len(imgs)) if i not in set(wide)]
+                if wide and getattr(self.settings, "show_patch_results", False):
+                    raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
+                if center3d_override is not None:
+                    assert center3d_override.shape[0] >= len(normal)
+                res = [None] * len(imgs)
+                for c0 in range(0, max(len(normal), 1), self.max_batch):
+                    idx = normal[c0:c0 + self.max_batch]
+                    last = c0 + self.max_batch >= len(normal)
+                    now = [i for i in wide if last or i < idx[0]]
+                    wide = wide[len(now):]
+                    co = None if center3d_override is None or not idx else center3d_override[c0:c0 + len(idx)]
+                    yield imgs, sids, res, idx, co, now, last
+
+        pending = None
+        for imgs, sids, res, idx, co, wide, last in chunks():
+            if wide and pending is not None:       # drain: the long-image mode runs in the current slot's rows
+                done = self._finish_images(*pending, to_numpy)
+                pending = None
+                if done is not None:
+                    yield done
+            for i in wide:
+                res[i] = self.process_long_image(imgs[i], to_numpy=to_numpy)
+            slot = self._submit_images([imgs[i] for i in idx], co, [sids[i] for i in idx]) if idx else None
+            if pending is not None:
+                done = self._finish_images(*pending, to_numpy)
+                if done is not None:
+                    yield done
+            pending = (slot, res, idx, last)
+        if pending is not None:
+            yield self._finish_images(*pending, to_numpy)
+
+    def _submit_images(self, imgs, center3d_override, signal_IDs):
+        """One chunk of normal images into the next slot: host images staged into its pinned buffer and sent with one H2D
+        on the copy stream, one preprocessing kernel into its frames and pad table, then the chunk's kernels."""
         B = len(imgs)
-        # the previous chunk ended in a host sync: the pinned buffer is free, and self.stream is the last reader of both
-        offs, total = self.raw.stage(imgs, replace_after=self.stream)
+        slot = self._next_slot()
+        fd = frame_buffer(slot["frames"], torch.uint8, B, self.tdevice)
+        raw = slot["raw"]
+        offs, total = raw.stage(imgs, replace_after=slot["done"], reuse_after=slot["h2d"])
+        if total:
+            with torch.cuda.stream(self.copy_stream):
+                self.copy_stream.wait_event(slot["done"])      # the slot's previous preprocessing no longer reads raw.dev
+                raw.upload(total)
+                slot["h2d"].record(self.copy_stream)
+            self.stream.wait_event(slot["h2d"])
         after_producers(self.stream, self.tdevice, *imgs)
-        fd = frame_buffer(self._frames, torch.uint8, B, self.tdevice)
         with torch.cuda.stream(self.stream):
-            if total:
-                self.raw.upload(total)
-            preprocess_bgr_batch(self.lib, imgs, offs, self.raw.dev, fd, self.pad_table, self.stream.cuda_stream)
-            self.run_model(fd, center3d_override)
-            if self.temporal:
-                self.run_temporal(B, signal_IDs)
-                self.run_post_temporal(B, self.pad_table[:B])
-            else:
-                self.run_post(B, self.pad_table[:B])
-        if self.temporal:
-            out, rows = self._collect_temporal(B, to_numpy)
-            return self._split_temporal(out, B, rows, to_numpy)
-        out = self.collect(to_numpy)
-        if out is None:
-            return [None] * B
-        n_det = int(self.count_host[0])
-        detected = set(self.buf["batch_ids"][:n_det].cpu().tolist())       # frames with a detection (before the filters)
-        res = split_by_frame(out, B, to_numpy)
-        for i, r in enumerate(res):
-            n = len(r["cam"])
-            r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
-        return [r if i in detected else None for i, r in enumerate(res)]      # an undetected frame alone returns None
+            preprocess_bgr_batch(self.lib, imgs, offs, raw.dev, fd, slot["pad"], self.stream.cuda_stream)
+            self._run(slot, fd, B, slot["pad"][:B], 512.0, center3d_override, signal_IDs)
+        return slot
+
+    def _finish_images(self, slot, res, idx, last, to_numpy):
+        """Read back one chunk into res at its images' places; returns res once its list's last chunk is in."""
+        if slot is not None:
+            for i, r in zip(idx, self._per_frame(self._read_back(slot, len(idx), to_numpy, self.temporal, True), len(idx), to_numpy)):
+                res[i] = r
+        return res if last else None
 
     def _long_buffers(self, rows):
         """Image-level accumulation rows of the long-image mode (grown on demand, kept for the next image)."""
@@ -533,7 +675,7 @@ class BEV(torch.nn.Module):
             after_producers(self.stream, self.tdevice, center3d_override)
         lb = self._long_buffers(K * MAX_PERSON)
         tab = torch.from_numpy(long_image_crop_table(boxes, pad_length, h, w, float(s.nms_thresh))).pin_memory()
-        frames = frame_buffer(self._frames, torch.uint8, B, self.tdevice)
+        frames = frame_buffer(self.slots[self._slot]["frames"], torch.uint8, B, self.tdevice)     # free: callers drain first
         with torch.cuda.stream(self.stream):
             padded = self.pad_long_image(img, pad_length)
             tab_dev = tab.to(self.tdevice, non_blocking=True)
@@ -596,7 +738,11 @@ class BEV(torch.nn.Module):
         if n_det == 0:                        # the reference raises KeyError here (main.py:253); INTEGRATION.md, Deviations
             print("No person detected!")
             return None
-        return self._result(lb["out"], n, torch.zeros(n, dtype=torch.int64, device=self.tdevice), to_numpy)
+        out = self._result(lb["out"], n, torch.zeros(n, dtype=torch.int64, device=self.tdevice))
+        if to_numpy:
+            with torch.cuda.stream(self.stream):
+                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
+        return out
 
     @torch.no_grad()
     def forward(self, image, signal_ID=0, **kwargs):

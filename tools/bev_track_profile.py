@@ -1,16 +1,20 @@
-"""Time BEV's video mode (-t) on a seeded synthetic video: 256 frames, 10-30 moving people planted through
+"""Time BEV's image path and video mode (-t) on a seeded synthetic video: 256 frames, 10-30 moving people planted through
 center3d_override, synthetic weights.
 
     python tools/bev_track_profile.py [--precision bf16] [--batch 32] [--iters 3]
 
-Reports (median of --iters runs after one warm-up run of each):
-  frames_per_s_t        : BEV.forward_images(frames, center3d_override=...) with -t, in chunks of --batch frames (numpy in,
-                          per-frame dicts out; host wall clock, each chunk ends in its stream sync);
-  frames_per_s_plain    : the same call on an instance without -t;
+Reports (median of --iters runs after one warm-up run of each), for an instance without -t (``plain``) and one with it (``t``):
+  frames_per_s_<m>       : BEV.forward_images(chunk, center3d_override=...) called once per chunk of --batch frames (numpy in,
+                           per-frame dicts out; host wall clock), each call ending in its own read-back;
+  frames_per_s_<m>_stream: BEV.forward_image_batches([frames]) over the whole video: the same chunks on the two-slot pipeline,
+                           staging and read-back of neighbouring chunks overlapping each chunk's kernels;
+  device_ms_per_chunk_<m>: CUDA events on the BEV stream from each chunk's run_model to the end of its run_post (the chunk's
+                           device work after the preprocessing kernel), median over the chunk loop's chunks;
+  wall_ms_per_chunk_<m>[_stream]: host wall clock per chunk of the two calls above;
   track_kernel_us_per_frame : CUDA events on the BEV stream around b200romp_bev_track_step, summed over the video / frames;
   oracle_cpu_us_per_frame  : CPU figure, for context: oracle/track_oracle.py (numpy, the reference's algorithm) stepping
-                          the same video's parse outputs on the host;
-  extra_device_mb       : device memory a -t instance allocates beyond a plain one at this --batch.
+                           the same video's parse outputs on the host;
+  extra_device_mb        : device memory a -t instance allocates beyond a plain one at this --batch.
 The card name and power limit (read-only queries) are printed beside the numbers.
 """
 import argparse
@@ -76,73 +80,98 @@ def volumes(cells, seed):
     return vol
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--precision", default="bf16", choices=["bf16", "tf32", "fp32"])
-    ap.add_argument("--batch", type=int, default=32)
-    ap.add_argument("--frames", type=int, default=256)
-    ap.add_argument("--iters", type=int, default=3)
-    a = ap.parse_args()
-    T, B = a.frames, a.batch
-    params = dict(state_dict=synth.bev_damp_cam_offsets(synth.bev_state_dict(0)), smpla_pack=synth.smpl_pack(0, num_betas=11),
-                  smil_pack=synth.smpl_pack(1))
-    cells = trajectories(T, 0)
-    counts = [len(c) for c in cells]
-    img = np.random.RandomState(1).randint(0, 256, (480, 640, 3)).astype(np.uint8)
-    imgs = [img] * T
-    vols = [volumes(cells[c0:c0 + B], c0) for c0 in range(0, T, B)]
-    flags = ["--precision", a.precision, "--max_batch", str(B)]
+def instrument(m):
+    """CUDA events on m.stream: from each chunk's run_model to the end of its run_post, and around every track step."""
+    spans = dict(chunk=[], track=[])
+
+    def wrap(name, opens, closes):
+        f = getattr(m, name)
+
+        def timed(*args, **kw):
+            if opens:
+                spans[opens].append([torch.cuda.Event(enable_timing=True), None])
+                spans[opens][-1][0].record(m.stream)
+            r = f(*args, **kw)
+            if closes:
+                spans[closes][-1][1] = torch.cuda.Event(enable_timing=True)
+                spans[closes][-1][1].record(m.stream)
+            return r
+        setattr(m, name, timed)
+    wrap("run_model", "chunk", None)
+    wrap("run_post", None, "chunk")
+    if m.temporal:
+        wrap("run_temporal", "track", "track")
+    return spans
+
+
+def elapsed_ms(spans):
     torch.cuda.synchronize()
-    m0 = torch.cuda.memory_allocated()
-    plain = BEV(bev_settings(flags), **params)
-    m1 = torch.cuda.memory_allocated()
-    tm = BEV(bev_settings(flags + ["-t"]), **params)
-    m2 = torch.cuda.memory_allocated()
+    return [e0.elapsed_time(e1) for e0, e1 in spans]
 
-    # the track kernel's device time: CUDA events on the BEV stream around every step
-    spans = []
-    run_temporal = tm.run_temporal
 
-    def timed_run_temporal(*args):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(tm.stream)
-        run_temporal(*args)
-        e1.record(tm.stream)
-        spans.append((e0, e1))
-    tm.run_temporal = timed_run_temporal
+class Video:
+    """The seeded 256-frame video and the two ways of running it through a BEV instance."""
 
-    def video(m):
-        if m is tm:
+    def __init__(self, T, B):
+        self.T, self.B = T, B
+        self.cells = trajectories(T, 0)
+        img = np.random.RandomState(1).randint(0, 256, (480, 640, 3)).astype(np.uint8)
+        self.img, self.imgs = img, [img] * T
+        self.vol = torch.cat([volumes(self.cells[c0:c0 + B], c0) for c0 in range(0, T, B)])
+
+    def loop(self, m):
+        """forward_images once per chunk: wall seconds, per-frame results"""
+        if m.temporal:
             m.reset_temporal()
         out, t0 = [], time.perf_counter()
-        for k, c0 in enumerate(range(0, T, B)):
-            out += m.forward_images(imgs[c0:c0 + B], center3d_override=vols[k])
+        for c0 in range(0, self.T, self.B):
+            out += m.forward_images(self.imgs[c0:c0 + self.B], center3d_override=self.vol[c0:c0 + self.B])
         return time.perf_counter() - t0, out
 
-    res = {}
-    for name, m in (("plain", plain), ("t", tm)):
-        video(m)                                                             # warm-up: graphs, staging buffers
-        ts, kern = [], []
-        for _ in range(a.iters):
-            spans.clear()
-            dt, out = video(m)
+    def stream(self, m):
+        """forward_image_batches over the whole video as one list (the same chunks, pipelined)"""
+        if m.temporal:
+            m.reset_temporal()
+        t0 = time.perf_counter()
+        out = next(m.forward_image_batches([self.imgs], center3d_override=self.vol))
+        return time.perf_counter() - t0, out
+
+
+def measure(v, m, name, iters, res, stream=True):
+    """frame rates, wall and device time per chunk of instance m into res (keys suffixed with name)"""
+    spans = instrument(m)
+    chunks = -(-v.T // v.B)
+    for how in ("loop", "stream") if stream else ("loop",):
+        run = getattr(v, how)
+        run(m)                                                               # warm-up: graphs, staging buffers, mirrors
+        ts, dev, kern = [], [], []
+        for _ in range(iters):
+            spans["chunk"].clear()
+            spans["track"].clear()
+            dt, out = run(m)
             ts.append(dt)
-            if m is tm:
-                torch.cuda.synchronize()
-                kern.append(sum(e0.elapsed_time(e1) for e0, e1 in spans) * 1e3 / T)
-        res[f"frames_per_s_{name}"] = round(T / float(np.median(ts)), 1)
-        if m is tm:
+            dev += elapsed_ms(spans["chunk"])
+            kern.append(sum(elapsed_ms(spans["track"])) * 1e3 / v.T)
+        sfx = name if how == "loop" else name + "_stream"
+        res[f"frames_per_s_{sfx}"] = round(v.T / float(np.median(ts)), 1)
+        res[f"wall_ms_per_chunk_{sfx}"] = round(float(np.median(ts)) * 1e3 / chunks, 2)
+        res[f"device_ms_per_chunk_{sfx}"] = round(float(np.median(dev)), 2)
+        if m.temporal and how == "loop":
             res["track_kernel_us_per_frame"] = round(float(np.median(kern)), 2)
             res["rows_out"] = int(sum(0 if o is None else len(o["track_ids"]) for o in out))
             res["ids"] = int(len({i for o in out if o is not None for i in o["track_ids"].tolist()}))
+    return spans
 
-    # CPU figure: the oracle tracker on the same parse outputs (read from a plain instance's device rows)
+
+def oracle_cpu_us_per_frame(v, plain, iters):
+    """The oracle tracker on the video's parse outputs (read from a plain instance's device rows), host time per frame."""
     parsed = []
-    for k, c0 in enumerate(range(0, T, B)):
+    T, B = v.T, v.B
+    for c0 in range(0, T, B):
         nb = min(B, T - c0)
-        frames = torch.from_numpy(np.ascontiguousarray(np.repeat(img_preprocess(img)[0], nb, 0))).cuda()
+        frames = torch.from_numpy(np.ascontiguousarray(np.repeat(img_preprocess(v.img)[0], nb, 0))).cuda()
         with torch.cuda.stream(plain.stream):
-            plain.run_model(frames, vols[k])
+            plain.run_model(frames, v.vol[c0:c0 + nb])
         plain.stream.synchronize()
         n = int(plain.buf["count"].item())
         b = {key: plain.buf[src][:n].cpu().numpy() for key, src in (("smpl_thetas", "thetas"), ("smpl_betas", "betas"), ("cam", "cam"),
@@ -150,18 +179,45 @@ def main():
                                                                      ("center_confs", "conf"), ("pred_batch_ids", "batch_ids"))}
         for f in range(nb):
             sel = b["pred_batch_ids"] == f
-            parsed.append({key: v[sel] for key, v in b.items()} if sel.any() else {})
+            parsed.append({key: x[sel] for key, x in b.items()} if sel.any() else {})
     host = []
-    for _ in range(a.iters):
+    for _ in range(iters):
         sm = TO.TemporalBEV()
         t0 = time.perf_counter()
         for f in parsed:
             if f:
                 sm(f, 0)
         host.append((time.perf_counter() - t0) * 1e6 / T)
-    res["oracle_cpu_us_per_frame"] = round(float(np.median(host)), 1)
+    return round(float(np.median(host)), 1)
+
+
+def params():
+    return dict(state_dict=synth.bev_damp_cam_offsets(synth.bev_state_dict(0)), smpla_pack=synth.smpl_pack(0, num_betas=11),
+                smil_pack=synth.smpl_pack(1))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--precision", default="bf16", choices=["bf16", "tf32", "fp32"])
+    ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--frames", type=int, default=256)
+    ap.add_argument("--iters", type=int, default=3)
+    a = ap.parse_args()
+    v = Video(a.frames, a.batch)
+    flags = ["--precision", a.precision, "--max_batch", str(a.batch)]
+    torch.cuda.synchronize()
+    m0 = torch.cuda.memory_allocated()
+    plain = BEV(bev_settings(flags), **params())
+    m1 = torch.cuda.memory_allocated()
+    tm = BEV(bev_settings(flags + ["-t"]), **params())
+    m2 = torch.cuda.memory_allocated()
+    res = {}
+    measure(v, plain, "plain", a.iters, res)
+    measure(v, tm, "t", a.iters, res)
+    res["oracle_cpu_us_per_frame"] = oracle_cpu_us_per_frame(v, plain, a.iters)
     name, power = card()
-    res.update(people_per_frame=[min(counts), max(counts)], frames=T, batch=B, precision=a.precision,
+    counts = [len(c) for c in v.cells]
+    res.update(people_per_frame=[min(counts), max(counts)], frames=v.T, batch=v.B, precision=a.precision,
                extra_device_mb=round(((m2 - m1) - (m1 - m0)) / 2**20, 1), gpu=name, power_limit=power, iters=a.iters)
     print(json.dumps(res))
 
