@@ -162,6 +162,20 @@ __device__ __forceinline__ void wgmma_n128_bf16(float (&d)[64], uint64_t a, uint
       : "l"(a), "l"(b), "r"(scale_d)
       : "memory");
 }
+// bf16 only: conv1 of the folded BasicBlock (conv_block_tc.cu), 192 mid pixels per warpgroup
+__device__ __forceinline__ void wgmma_n192_bf16(float (&d)[96], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
+      "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
+      "%63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, "
+      "%87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, 0, 0;\n\t}"
+      : B2R_WG_R8(0), B2R_WG_R8(8), B2R_WG_R8(16), B2R_WG_R8(24), B2R_WG_R8(32), B2R_WG_R8(40), B2R_WG_R8(48), B2R_WG_R8(56),
+        B2R_WG_R8(64), B2R_WG_R8(72), B2R_WG_R8(80), B2R_WG_R8(88)
+      : "l"(a), "l"(b), "r"(scale_d)
+      : "memory");
+}
 #undef B2R_WG_R8
 template <int NT, int EB>
 __device__ __forceinline__ void wgmma_any(float (&d)[NT / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
