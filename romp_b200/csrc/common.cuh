@@ -141,6 +141,8 @@ struct SumParams {
   int B, H, W, C, relu;
 };
 int launch_fuse_sum(const SumParams& p, cudaStream_t stream);
+// the kernel launch_fuse_sum takes for p ("ring", "pipe" or "simple"): it depends on the pointers' alignment, so p must be bound
+const char* fuse_sum_kernel_name(const SumParams& p);
 
 // engines implemented in other translation units
 int launch_conv_simt(const ConvParams& p, int ksize, int stride, cudaStream_t stream);

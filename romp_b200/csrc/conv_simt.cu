@@ -513,52 +513,76 @@ __global__ void __launch_bounds__(256) fuse_sum_ring_kernel(const SumParams p, c
   (void)ES;
 }
 
+// Which fuse-sum kernel runs p: the pipe kernel when every tensor has the base's dtype and a base row fits the ring, the ring
+// kernel instead when B200ROMP_SUM_RING=1 and every term is a whole tensor (no channel slice) with 16-byte rows (*ring then
+// holds its stage layout), else the one-chunk-per-thread kernel (always with B200ROMP_SUM_SIMPLE=1).
+enum class SumKernel { Simple, Pipe, Ring };
+static SumKernel choose_fuse_sum(const SumParams& p, SumRingCfg* ring, int* ring_blocks_per_sm) {
+  const int per_row = p.W * (p.C / 8);
+  const int row_bytes = p.W * p.C * (int)dtype_size(p.base_dt);
+  static const bool no_pipe = [] { const char* e = getenv("B200ROMP_SUM_SIMPLE"); return e && e[0] == '1'; }();
+  bool same_dt = p.out_dt == p.base_dt;
+  for (int k = 0; k < p.n_terms; ++k) same_dt = same_dt && p.term_dt[k] == p.base_dt;
+  const bool pipe_ok = !no_pipe && same_dt && row_bytes % 16 == 0 && row_bytes <= 16384 && (reinterpret_cast<uintptr_t>(p.base) & 15) == 0 && per_row >= 128;
+  if (!pipe_ok) return SumKernel::Simple;
+  static const bool want_ring = [] { const char* e = getenv("B200ROMP_SUM_RING"); return e && e[0] == '1'; }();
+  if (!want_ring) return SumKernel::Pipe;
+  // every term a whole tensor (no channel slice) whose rows are 16-byte multiples: all operands travel through the ring
+  SumRingCfg cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  bool ok = true;
+  int off = row_bytes;
+  const int es = (int)dtype_size(p.base_dt);
+  for (int k = 0; k < p.n_terms; ++k) {
+    ok = ok && p.term_C[k] == p.C && p.term_c_off[k] == 0 && (reinterpret_cast<uintptr_t>(p.term[k]) & 15) == 0;
+    cfg.term_bytes[k] = (p.W / p.up[k]) * p.C * es;
+    ok = ok && cfg.term_bytes[k] % 16 == 0;
+    cfg.term_off[k] = off;
+    off += cfg.term_bytes[k];
+  }
+  cfg.stage_bytes = (off + 127) / 128 * 128;
+  const int blocks_per_sm = cfg.stage_bytes <= 21 * 1024 ? 3 : 2;
+  cfg.stages = std::min(4, (200 * 1024 / blocks_per_sm - 256) / cfg.stage_bytes);
+  if (!ok || cfg.stages < 2) return SumKernel::Pipe;
+  if (ring) *ring = cfg;
+  if (ring_blocks_per_sm) *ring_blocks_per_sm = blocks_per_sm;
+  return SumKernel::Ring;
+}
+
+const char* fuse_sum_kernel_name(const SumParams& p) {
+  switch (choose_fuse_sum(p, nullptr, nullptr)) {
+    case SumKernel::Ring: return "ring";
+    case SumKernel::Pipe: return "pipe";
+    default: return "simple";
+  }
+}
+
 int launch_fuse_sum(const SumParams& p, cudaStream_t stream) {
   const int c8n = p.C / 8;
   auto lg = [](int u) { return u == 8 ? 3 : u == 4 ? 2 : u == 2 ? 1 : 0; };
   const int4 sh = make_int4(lg(p.up[0]), lg(p.up[1]), lg(p.up[2]), lg(p.up[3]));
   const int per_row = p.W * c8n;
   const int row_bytes = p.W * p.C * (int)dtype_size(p.base_dt);
-  static const bool no_pipe = [] { const char* e = getenv("B200ROMP_SUM_SIMPLE"); return e && e[0] == '1'; }();
-  bool same_dt = p.out_dt == p.base_dt;
-  for (int k = 0; k < p.n_terms; ++k) same_dt = same_dt && p.term_dt[k] == p.base_dt;
-  const bool pipe_ok = !no_pipe && same_dt && row_bytes % 16 == 0 && row_bytes <= 16384 && (reinterpret_cast<uintptr_t>(p.base) & 15) == 0 && per_row >= 128;
   int c8_shift = -1;
   for (int b2 = 0; b2 < 8; ++b2) if ((1 << b2) == c8n) c8_shift = b2;
-  static const bool want_ring = [] { const char* e = getenv("B200ROMP_SUM_RING"); return e && e[0] == '1'; }();
-  if (pipe_ok && want_ring) {
-    // every term a whole tensor (no channel slice) whose rows are 16-byte multiples: all operands travel through the ring
-    SumRingCfg cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    bool ok = true;
-    int off = row_bytes;
-    const int es = (int)dtype_size(p.base_dt);
-    for (int k = 0; k < p.n_terms; ++k) {
-      ok = ok && p.term_C[k] == p.C && p.term_c_off[k] == 0 && (reinterpret_cast<uintptr_t>(p.term[k]) & 15) == 0;
-      cfg.term_bytes[k] = (p.W / p.up[k]) * p.C * es;
-      ok = ok && cfg.term_bytes[k] % 16 == 0;
-      cfg.term_off[k] = off;
-      off += cfg.term_bytes[k];
+  SumRingCfg cfg;
+  int ring_blocks_per_sm = 0;
+  const SumKernel kernel = choose_fuse_sum(p, &cfg, &ring_blocks_per_sm);
+  if (kernel == SumKernel::Ring) {
+    const int smem = cfg.stages * cfg.stage_bytes + 2 * cfg.stages * 8 + 128;
+    static bool ring_attr = false;
+    if (!ring_attr) {
+      B2R_CUDA_OK(cudaFuncSetAttribute(fuse_sum_ring_kernel<B200ROMP_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
+      B2R_CUDA_OK(cudaFuncSetAttribute(fuse_sum_ring_kernel<B200ROMP_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
+      ring_attr = true;
     }
-    cfg.stage_bytes = (off + 127) / 128 * 128;
-    const int blocks_per_sm = cfg.stage_bytes <= 21 * 1024 ? 3 : 2;
-    cfg.stages = std::min(4, (200 * 1024 / blocks_per_sm - 256) / cfg.stage_bytes);
-    if (ok && cfg.stages >= 2) {
-      const int smem = cfg.stages * cfg.stage_bytes + 2 * cfg.stages * 8 + 128;
-      static bool ring_attr = false;
-      if (!ring_attr) {
-        B2R_CUDA_OK(cudaFuncSetAttribute(fuse_sum_ring_kernel<B200ROMP_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-        B2R_CUDA_OK(cudaFuncSetAttribute(fuse_sum_ring_kernel<B200ROMP_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-        ring_attr = true;
-      }
-      const int grid = std::min(p.B * p.H, 132 * blocks_per_sm);
-      if (p.base_dt == B200ROMP_F32) fuse_sum_ring_kernel<B200ROMP_F32><<<grid, 256, smem, stream>>>(p, cfg, c8n, c8_shift, sh, row_bytes);
-      else fuse_sum_ring_kernel<B200ROMP_BF16><<<grid, 256, smem, stream>>>(p, cfg, c8n, c8_shift, sh, row_bytes);
-      B2R_CUDA_OK(cudaGetLastError());
-      return B200ROMP_OK;
-    }
+    const int grid = std::min(p.B * p.H, 132 * ring_blocks_per_sm);
+    if (p.base_dt == B200ROMP_F32) fuse_sum_ring_kernel<B200ROMP_F32><<<grid, 256, smem, stream>>>(p, cfg, c8n, c8_shift, sh, row_bytes);
+    else fuse_sum_ring_kernel<B200ROMP_BF16><<<grid, 256, smem, stream>>>(p, cfg, c8n, c8_shift, sh, row_bytes);
+    B2R_CUDA_OK(cudaGetLastError());
+    return B200ROMP_OK;
   }
-  if (pipe_ok) {
+  if (kernel == SumKernel::Pipe) {
     const int smem = kSumStages * row_bytes + 2 * kSumStages * 8 + 128;
     static bool attr_done = false;
     if (!attr_done) {

@@ -882,7 +882,14 @@ int b200romp_net_describe(b200romp_net* net, char* buf, int len) {
       case Kernel::Sum: {
         int n = snprintf(line, sizeof(line), "op%03zu sum     out t%d[%dx%dx%d] = relu%d( t%d", i, op.sum.out, to.H, to.W, to.C, op.sum.relu, op.sum.base);
         for (int k = 0; k < op.sum.n_terms; ++k) n += snprintf(line + n, sizeof(line) - n, " + up%d(t%d)", op.sum.up[k], op.sum.term[k]);
-        snprintf(line + n, sizeof(line) - n, " )\n");
+        n += snprintf(line + n, sizeof(line) - n, " )");
+        // the kernel follows from the tensors' addresses: named once every tensor of the sum is bound
+        bool bound = net->finalized && to.ptr && ti.ptr;
+        for (int k = 0; k < op.sum.n_terms; ++k) bound = bound && net->tensors[op.sum.term[k]].ptr;
+        SumParams sp;
+        if (bound && fill_sum_params(net, op, net->max_batch, &sp) == B200ROMP_OK)
+          n += snprintf(line + n, sizeof(line) - n, " [fuse-sum %s]", fuse_sum_kernel_name(sp));
+        snprintf(line + n, sizeof(line) - n, "\n");
         s += line;
         break;
       }
