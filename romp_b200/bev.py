@@ -24,7 +24,7 @@ import torch
 from . import _lib, graph
 from ._lib import BF16, F32, U8
 from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
-from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch
+from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, to_caller
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
 long_conf_dict = {1: [0.12, 20, 1.5, 0.46], 2: [0.08, 20, 1.6, 0.8]}
@@ -442,10 +442,11 @@ class BEV(torch.nn.Module):
         """forward_batch's dict from a read-back: host arrays, or device views"""
         return None if got is None else got[0]
 
-    def _per_frame(self, got, B, to_numpy):
-        """forward_images' per-frame dicts from a chunk's read-back: None for a frame without a result, else the frame's
-        rows of every key (arrays that own their memory, or device copies) with pred_batch_ids zeroed.  The rows come in
-        frame order, so each frame's rows are one host searchsorted on their frame ids."""
+    def _per_frame(self, got, B, to_numpy, slot):
+        """forward_images' per-frame dicts from a chunk's read-back in ``slot``: None for a frame without a result, else
+        the frame's rows of every key (arrays that own their memory, or device copies on the caller's stream) with
+        pred_batch_ids zeroed.  The rows come in frame order, so each frame's rows are one host searchsorted on their
+        frame ids."""
         res = [None] * B
         if got is None:
             return res
@@ -453,17 +454,20 @@ class BEV(torch.nn.Module):
         br = np.searchsorted(rows, np.arange(B + 1)).tolist()
         bd = np.searchsorted(det, np.arange(B + 1)).tolist()
         largest = LARGEST_KEYS if self.temporal and self.show_largest else ()
-        with torch.cuda.stream(self.d2h_stream):
-            for f in frames:
-                r = {}
-                for k, v in out.items():
-                    s, e = (bd[f], bd[f + 1]) if k in largest else (br[f], br[f + 1])
-                    r[k] = np.array(v[s:e]) if to_numpy else v[s:e].clone()
-                n = len(r["pred_batch_ids"])
-                r["pred_batch_ids"] = np.zeros(n, np.int64) if to_numpy else torch.zeros(n, dtype=torch.int64, device=self.tdevice)
-                res[f] = r
+        for f in frames:
+            r = {}
+            for k, v in out.items():
+                s, e = (bd[f], bd[f + 1]) if k in largest else (br[f], br[f + 1])
+                r[k] = np.array(v[s:e]) if to_numpy else v[s:e]
+            res[f] = r
         if not to_numpy:
-            self.d2h_stream.synchronize()           # the copies have read the slot before its next chunk overwrites it
+            res = to_caller(res, slot["done"], self.stream)
+        for r in res:
+            if r is not None:
+                if to_numpy:
+                    r["pred_batch_ids"] = np.zeros(len(r["pred_batch_ids"]), np.int64)
+                else:
+                    r["pred_batch_ids"].zero_()
         return res
 
     def collect(self, to_numpy=True):
@@ -496,7 +500,7 @@ class BEV(torch.nn.Module):
         for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
         suppressing with its own max(h, w) (``img_max_side`` is not used).  With -t the frames are consecutive video
         frames, tracked and smoothed in order (``signal_IDs``: one per frame, default 0); the result adds ``track_ids``.
-        ``to_numpy=False`` returns device views of the slot's rows, valid until the second-next batch."""
+        ``to_numpy=False`` returns device tensors of the caller's current stream (see forward_batches)."""
         sids = None if signal_IDs is None else [signal_IDs]
         return next(self.forward_batches([frames], offsets, center3d_override, to_numpy, img_max_side, sids))
 
@@ -506,18 +510,28 @@ class BEV(torch.nn.Module):
         ``forward_batch`` returns for each batch, in order.  Each batch goes into the next of two slots: its frames are
         copied into the slot's frame buffer on the copy stream, so the copy of batch i+1 and the read-back of batch i-1
         overlap the kernels of batch i.  The generator goes on once a host batch has been copied, so a caller may refill
-        one pinned buffer between batches.  ``offsets``, ``center3d_override`` and ``img_max_side`` apply to every batch;
-        with -t the batches are consecutive parts of one video and ``signal_IDs`` is None or one sequence per batch."""
+        one (pinned or numpy) buffer in place between batches.  ``offsets``, ``center3d_override`` and ``img_max_side``
+        apply to every batch; with -t the batches are consecutive parts of one video and ``signal_IDs`` is None or one
+        sequence per batch.  Device-resident frames, ``center3d_override`` and per-frame ``offsets`` may come from
+        producers on the caller's current stream (the model's streams wait for it) and may be dropped once handed over.
+        The yielded results own their memory: arrays, or with ``to_numpy=False`` copies made on the caller's current
+        stream after the batch's kernels, which the caller may read there at any later time (the model's kernels wait
+        for the copies before they reuse the slot)."""
         after_producers(self.stream, self.tdevice, center3d_override, offsets)
         sid_iter = None if signal_IDs is None else iter(signal_IDs)
         pending = None
         for frames in batches:
             slot = self._submit_frames(frames, offsets, center3d_override, img_max_side, None if sid_iter is None else next(sid_iter))
             if pending is not None:
-                yield self._batch(self._read_back(*pending, to_numpy, self.temporal))
+                yield self._batch_result(*pending, to_numpy)
             pending = slot
         if pending is not None:
-            yield self._batch(self._read_back(*pending, to_numpy, self.temporal))
+            yield self._batch_result(*pending, to_numpy)
+
+    def _batch_result(self, slot, B, to_numpy):
+        """A batch's result for the caller: arrays (to_numpy), else copies of the slot's rows on the caller's stream."""
+        out = self._batch(self._read_back(slot, B, to_numpy, self.temporal))
+        return out if out is None or to_numpy else to_caller([out], slot["done"], self.stream)[0]
 
     def _submit_frames(self, frames, offsets, center3d_override, img_max_side, signal_IDs):
         """One batch of frames into the next slot; returns (slot, B) once host frames have been copied."""
@@ -562,7 +576,9 @@ class BEV(torch.nn.Module):
         wide crowd-mode image drains the pipeline and runs through ``process_long_image`` between its list's chunks.
         center3d_override applies to every list, entry k to the k-th normal image of the list.  With -t the lists are
         consecutive parts of one video (tracker and filters carry across them) and ``signal_IDs`` is None or one sequence
-        per list."""
+        per list.  Host images have been staged when the generator pulls the next list; device images and
+        ``center3d_override`` may come from producers on the caller's current stream.  The yielded results own their
+        memory, as in ``forward_batches``."""
         if center3d_override is not None:
             assert center3d_override.is_cuda
         after_producers(self.stream, self.tdevice, center3d_override)
@@ -632,7 +648,7 @@ class BEV(torch.nn.Module):
     def _finish_images(self, slot, res, idx, last, to_numpy):
         """Read back one chunk into res at its images' places; returns res once its list's last chunk is in."""
         if slot is not None:
-            for i, r in zip(idx, self._per_frame(self._read_back(slot, len(idx), to_numpy, self.temporal, True), len(idx), to_numpy)):
+            for i, r in zip(idx, self._per_frame(self._read_back(slot, len(idx), to_numpy, self.temporal, True), len(idx), to_numpy, slot)):
                 res[i] = r
         return res if last else None
 

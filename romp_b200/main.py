@@ -22,7 +22,8 @@ import torch
 
 from . import _lib, graph
 from ._lib import BF16, F32, U8
-from .staging import FULL_FRAME, RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, split_by_frame
+from .staging import (FULL_FRAME, RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch,
+                      split_by_frame, to_caller)
 
 MAX_PERSON = 64          # CenterMap.max_person, post_parser.py:11
 N_PARAMS = 145           # 3 cam + 22*6 rot6d + 10 betas, model.py:429
@@ -410,22 +411,31 @@ class ROMP(torch.nn.Module):
         padded+resized like img_preprocess.  Returns the reference's dict plus ``pred_batch_ids`` or None.
         ``offsets``: the pad info [top,bottom,left,right,h,w] of every frame, or one row per frame ([B,6], numpy or
         tensor) when the frames come from images of different sizes.
-        Device-resident ``frames`` / ``center_override`` may come straight from a producer on the caller's current
-        stream.  ``own=True`` (default) returns arrays that own their memory; ``own=False`` returns views of the pinned
-        read-back mirrors, valid until the second-next batch."""
+        Device-resident ``frames`` / ``center_override`` / ``offsets`` may come straight from a producer on the caller's
+        current stream.  ``own=True`` (default) returns arrays that own their memory; ``own=False`` returns views of the
+        pinned read-back mirrors, valid until the second-next batch.  ``to_numpy=False`` returns device tensors of the
+        caller's current stream (see forward_batches)."""
         after_producers(self.stream, self.tdevice, center_override, offsets)
-        out = self._read_back(self._submit_frames(frames, offsets, center_override), to_numpy)
+        out = self._result(self._submit_frames(frames, offsets, center_override), to_numpy)
         if out is not None and to_numpy and own:
             out = self._apply_cam_trans({k: np.array(v) for k, v in out.items()})
         return out
 
     @torch.no_grad()
     def forward_batches(self, batches, offsets=None, center_override=None, to_numpy=True, gather=None, frame_offset=0):
-        """Pipelined streaming over an iterable of host frame batches (video): yields one result dict (or None) per
-        batch, in order.  H2D of batch i+1 (copy stream) and D2H of batch i-1 (read-back stream) overlap the
-        kernels of batch i; the host waits only for the H2D copy of the batch it just handed over (so a caller may
-        refill one pinned buffer in a decode loop) and for the person count of an already finished batch.  With
-        ``to_numpy=True`` the yielded arrays are views of pinned mirrors, valid until the second-next batch is yielded.
+        """Pipelined streaming over an iterable of frame batches (video): yields one result dict (or None) per batch,
+        in order.  H2D of batch i+1 (copy stream) and D2H of batch i-1 (read-back stream) overlap the kernels of
+        batch i; the host waits only for the H2D copy of the batch it just handed over and for the person count of an
+        already finished batch.  Stream-order contract:
+        - a host batch has been copied when the generator pulls the next one, so a caller may refill one (pinned or
+          numpy) buffer in place in its decode loop;
+        - device-resident frames, ``center_override`` and per-frame ``offsets`` may come from producers on the caller's
+          current stream (the model's streams wait for it) and may be dropped right after they are handed over;
+        - with ``to_numpy=True`` the yielded arrays are views of pinned mirrors: they hold batch i until the generator
+          is resumed for batch i+2, whose read-back reuses them;
+        - with ``to_numpy=False`` the yielded tensors are copies made on the caller's current stream after the batch's
+          kernels: the caller may read them there at any later time, and the model's kernels wait for the copies
+          before they reuse the slot.
         Sharded (multi-GPU) use: pass ``gather`` (a shard.ShardGather built on ``record_layout()``) and this rank's
         ``frame_offset``; each batch's records are then packed and all-gathered on the gather's side stream right after
         its kernels, and the generator yields ``(own_result, gather_handle)`` pairs (own shard read back to this rank's
@@ -435,11 +445,11 @@ class ROMP(torch.nn.Module):
         for frames in batches:
             slot = self._submit_frames(frames, offsets, center_override, gather, frame_offset)
             if pending is not None:
-                res = self._read_back(pending, to_numpy)
+                res = self._result(pending, to_numpy)
                 yield (res, pending["gather"]) if gather is not None else res
             pending = slot
         if pending is not None:
-            res = self._read_back(pending, to_numpy)
+            res = self._result(pending, to_numpy)
             yield (res, pending["gather"]) if gather is not None else res
 
     def _submit_frames(self, frames, offsets, center_override, gather=None, frame_offset=0):
@@ -475,6 +485,11 @@ class ROMP(torch.nn.Module):
         self.d2h_stream.wait_event(slot["done"])
         return self.collect(to_numpy, slot, self.d2h_stream)   # device views stay valid until the slot's next batch
 
+    def _result(self, slot, to_numpy):
+        """A batch's result for the caller: arrays (to_numpy), else copies of the slot's rows on the caller's stream."""
+        out = self._read_back(slot, to_numpy)
+        return out if out is None or to_numpy else to_caller([out], slot["done"], self.stream)[0]
+
     @torch.no_grad()
     def forward_images(self, images, to_numpy=True, center_override=None):
         """Batched ``forward`` on raw images of any sizes: ``images`` is a sequence of HxWx3 uint8 BGR images (numpy arrays,
@@ -490,7 +505,10 @@ class ROMP(torch.nn.Module):
         on the copy stream (device images are read in place), preprocessed by one kernel into the slot's frames with
         a per-frame pad table, and post-processed with each frame's own geometry; staging chunk i+1 and reading back
         chunk i-1 overlap the kernels of chunk i (the two slots of ``forward_batches``).  center_override applies to
-        every list, entry k to the k-th image of the list."""
+        every list, entry k to the k-th image of the list.  Host images have been staged when the generator pulls the
+        next list; device images and ``center_override`` may come from producers on the caller's current stream.  The
+        yielded results own their memory: arrays, or with ``to_numpy=False`` device tensors copied on the caller's
+        current stream (as in ``forward_batches``)."""
         if self.temporal is not None:
             raise NotImplementedError("--temporal_optimize smooths one image sequence: call forward_video() (or forward() per frame)")
         after_producers(self.stream, self.tdevice, center_override)
@@ -554,7 +572,11 @@ class ROMP(torch.nn.Module):
         """Read back one chunk and scatter its persons to res[c0:c0+B]; returns res once its last chunk is in."""
         out = None if slot is None else self._read_back(slot, to_numpy)
         if out is not None:
-            for i, r in enumerate(split_by_frame(out, B, to_numpy)):
+            with torch.cuda.stream(self.d2h_stream):        # device frame ids are read after the slot's kernels
+                frames = split_by_frame(out, B, to_numpy)
+            if not to_numpy:
+                frames = to_caller(frames, slot["done"], self.stream)
+            for i, r in enumerate(frames):
                 if len(r["cam"]):
                     r.pop("pred_batch_ids")
                     res[c0 + i] = self._apply_cam_trans(r) if to_numpy else r
@@ -741,10 +763,11 @@ class ROMP(torch.nn.Module):
         else:
             per = {k: t[:n] for k, t in per.items()}
             rows = {k: t[:m] for k, t in rows.items()}
-            own = lambda t: t.clone()
+            own = lambda t: t                                # views, copied for the caller by to_caller below
         ids = lambda t: t.cpu().numpy() if isinstance(t, torch.Tensor) else t
-        pb = np.searchsorted(ids(per["ids"]), np.arange(B + 1)).tolist()
-        rb = np.searchsorted(ids(rows["ids"]), np.arange(B + 1)).tolist()
+        with torch.cuda.stream(st):                          # device frame ids are read after the slot's kernels
+            pb = np.searchsorted(ids(per["ids"]), np.arange(B + 1)).tolist()
+            rb = np.searchsorted(ids(rows["ids"]), np.arange(B + 1)).tolist()
         for i in range(B):
             s, e, a, z = pb[i], pb[i + 1], rb[i], rb[i + 1]
             if s == e:
@@ -755,7 +778,7 @@ class ROMP(torch.nn.Module):
             if tracked:
                 r["track_ids"] = own(per["track_ids"][s:e])
             res[i] = r
-        return res
+        return res if to_numpy else to_caller(res, slot["done"], self.stream)
 
     @torch.no_grad()
     def forward_video(self, images, signal_IDs=None, to_numpy=True, center_override=None):
@@ -775,7 +798,8 @@ class ROMP(torch.nn.Module):
         """Streaming form of ``forward_video`` over an iterable of image lists (consecutive parts of one video; the tracker
         state carries across lists): yields one result list per input list, in order, on forward_image_batches' two-slot
         pipeline.  ``signal_IDs``: None (every frame signal 0) or an iterable with one sequence of signal IDs per list.
-        center_override applies to every list, entry k to the k-th image of the list."""
+        center_override applies to every list, entry k to the k-th image of the list.  Inputs and results follow
+        ``forward_image_batches``: results own their memory (``to_numpy=False``: device copies on the caller's stream)."""
         if self.temporal is None:
             raise RuntimeError("forward_video needs -t/--temporal_optimize")
         after_producers(self.stream, self.tdevice, center_override)

@@ -56,11 +56,25 @@ def preprocess_bgr_batch(lib, images, offs, raw_dev, out, pad_table, stream):
 
 def split_by_frame(out, n_frames, to_numpy):
     """A batch result whose rows come in frame order -> one dict per frame with that frame's rows of every field
-    (possibly none): arrays that own their memory (to_numpy) or device copies."""
+    (possibly none): arrays that own their memory (to_numpy) or device views of ``out`` (for to_caller).  Device frame
+    ids are read on the current stream."""
     ids = out["pred_batch_ids"]
     ids = ids.cpu().numpy() if isinstance(ids, torch.Tensor) else ids
     b = np.searchsorted(np.asarray(ids), np.arange(n_frames + 1)).tolist()
-    return [{k: (np.array(v[s:e]) if to_numpy else v[s:e].clone()) for k, v in out.items()} for s, e in zip(b[:-1], b[1:])]
+    return [{k: (np.array(v[s:e]) if to_numpy else v[s:e]) for k, v in out.items()} for s, e in zip(b[:-1], b[1:])]
+
+
+def to_caller(results, done, stream):
+    """Device results (``to_numpy=False``) handed to the caller: ``results`` is a list of dicts of device views of a
+    slot's rows (or None), the slot's kernels end at the event ``done``, and ``stream`` writes the slot's next batch.
+    Returns copies made on the caller's current stream after ``done``, so that they belong to that stream like any
+    tensor the caller allocates there (the allocator recycles them in its order, not in the read-back's), and makes
+    ``stream`` wait for the copies before it overwrites the slot.  No host sync."""
+    cur = torch.cuda.current_stream(stream.device)
+    cur.wait_event(done)
+    out = [None if r is None else {k: v.clone() for k, v in r.items()} for r in results]
+    stream.wait_stream(cur)
+    return out
 
 
 def after_producers(stream, device, *tensors):
