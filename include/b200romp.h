@@ -358,6 +358,21 @@ int b200romp_bev_track_step(b200romp_bev_tracker* tracker, int batch, int capaci
                             float* out_betas, float* out_cam, float* out_cam_trans, float* out_params_pred, float* out_conf,
                             int* d_status, b200romp_stream stream);
 
+/* Stream mode (--video_streams): many independent videos in one batch.  A streams handle holds `streams` (1..
+ * B200ROMP_MAX_VIDEO_STREAMS) trackers, each with its own tracks, ids from 1, frame_id and filter set (max_tracks
+ * filter slots); no state is shared between streams.  b200romp_bev_track_step on it takes signal_slot[b] = the stream
+ * index of frame b in [0, streams) and steps every stream of the batch in parallel, one CTA per stream, each through its
+ * frames in batch order with the same per-frame step as above; rows come out grouped by frame, in frame order, with
+ * *d_out_count = total rows.  out_capacity must be at least 128 * batch (each frame's rows are first written to its
+ * own window of 128 rows, then compacted).  d_status = {frames whose stream failed, 0, then per frame its rows, or
+ * -1 = its stream's track table is full, -3 = its stream index is out of range}.  A full table fails only its stream:
+ * that stream's frames do nothing (status -1) until b200romp_bev_tracker_reset(tracker, stream) or (-1); every other
+ * stream steps normally.  Reset with signal = s >= 0 forgets stream s entirely (tracks, ids, frame_id, filters);
+ * -1 forgets every stream.  Device memory per stream: max_tracks * 1,292 + 20 bytes (165,396 at 128 tracks); shared memory per
+ * CTA: 104,592 bytes, so two CTAs fit on an SM. */
+#define B200ROMP_MAX_VIDEO_STREAMS 1024
+b200romp_bev_tracker* b200romp_bev_tracker_create_streams(int device, int max_tracks, int streams);
+
 /* ------------------------------------------------------------------------------------------------
  * ROMP's video mode for batches (ROMP.forward_video, -t/--temporal_optimize): the association and One-Euro smoothing of
  * ROMP.forward's per-frame temporal path (romp_b200/temporal.py TemporalState + b200romp_one_euro_smooth), decision for
@@ -384,6 +399,17 @@ int b200romp_romp_track_step(b200romp_romp_tracker* tracker, int batch, int capa
                              const float* cam, const float* thetas, const float* betas, const int* signal_code, int show_largest,
                              float smooth_coeff, float freq, int* d_out_count, long long* out_batch_ids, float* out_thetas,
                              float* out_betas, float* out_cam, int* out_slot, int* out_track_ids, b200romp_stream stream);
+
+/* Stream mode (--video_streams): a streams handle holds `streams` (1..B200ROMP_MAX_VIDEO_STREAMS) independent trackers,
+ * each with its own track table (ids from 1) and block of 64 filter slots; there is no registration by code and no
+ * eviction.  b200romp_romp_track_step on it takes signal_code[b] = the stream index of frame b in [0, streams) and
+ * steps every stream of the batch in parallel, one CTA per stream, each through its frames in batch order with the same
+ * per-frame step as above; out_slot is the slot within the stream's block (0..63, or -1).  The output rows keep the
+ * layout above.  Frames with an index out of range are left as they are.  b200romp_romp_tracker_reset forgets every
+ * stream, b200romp_romp_tracker_reset_stream stream s only.  Device memory per stream: 132,124 bytes; shared memory per
+ * CTA: 64,672 bytes. */
+b200romp_romp_tracker* b200romp_romp_tracker_create_streams(int device, int streams);
+int b200romp_romp_tracker_reset_stream(b200romp_romp_tracker* tracker, int s, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Frame-sharded multi-GPU collection (SURVEY 8e; the reference's DataParallel bookkeeping it stands in for:

@@ -172,6 +172,9 @@ def load():
     _sig(lib.b200romp_romp_tracker_destroy, None, vp)
     _sig(lib.b200romp_romp_tracker_reset, i32, vp, vp)
     _sig(lib.b200romp_romp_track_step, i32, vp, i32, i32, *([vp] * 6), i32, f32, f32, *([vp] * 7), vp)
+    _sig(lib.b200romp_bev_tracker_create_streams, vp, i32, i32, i32)
+    _sig(lib.b200romp_romp_tracker_create_streams, vp, i32, i32)
+    _sig(lib.b200romp_romp_tracker_reset_stream, i32, vp, i32, vp)
     _sig(lib.b200romp_preprocess_bgr, i32, vp, i32, i32, i32, i32, vp, fp, vp)
     _sig(lib.b200romp_preprocess_bgr_batch, i32, C.POINTER(vp), ip, ip, ip, i32, i32, vp, vp, vp)
     _sig(lib.b200romp_pack_rows, i32, C.POINTER(vp), ip, i32, vp, i32, i32, i32, i32, vp, i32, vp)
@@ -206,4 +209,5 @@ EXPORTS = [
     "b200romp_tracks_reset", "b200romp_one_euro_smooth",
     "b200romp_bev_tracker_create", "b200romp_bev_tracker_destroy", "b200romp_bev_tracker_reset", "b200romp_bev_track_step",
     "b200romp_romp_tracker_create", "b200romp_romp_tracker_destroy", "b200romp_romp_tracker_reset", "b200romp_romp_track_step",
+    "b200romp_bev_tracker_create_streams", "b200romp_romp_tracker_create_streams", "b200romp_romp_tracker_reset_stream",
 ]

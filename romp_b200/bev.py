@@ -24,6 +24,7 @@ import torch
 from . import _lib, graph
 from ._lib import BF16, F32, U8
 from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
+from .streams import MAX_VIDEO_STREAMS, check_streams, check_video_streams, stream_indices
 from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, to_caller
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
@@ -67,6 +68,11 @@ def bev_settings(input_args=sys.argv[1:]):
     p.add_argument("--webcam_id", type=int, default=0)
     p.add_argument("--precision", type=str, default="bf16", choices=["bf16", "tf32", "fp32"])
     p.add_argument("--max_batch", type=int, default=32)
+    # --- additions of this implementation (the reference has no equivalents)
+    p.add_argument("--video_streams", type=int, default=0,
+                   help=f"with -t: track up to N independent videos (one per signal_ID, each with its own tracker, ids and "
+                        f"filters), stepped in parallel on the GPU; 0 = one tracker shared by every signal_ID, like the "
+                        f"reference (at most {MAX_VIDEO_STREAMS})")
     args = p.parse_args(input_args)
     if args.model_id != 2:                                            # bev/main.py:59-63
         args.model_path = osp.join(home, model_dict[args.model_id])
@@ -132,6 +138,7 @@ class BEV(torch.nn.Module):
             raise NotImplementedError("display (--show) is outside the GPU hot path (SURVEY.md section 2)")
         self.temporal = bool(getattr(s, "temporal_optimize", False))
         self.show_largest = self.temporal and bool(getattr(s, "show_largest", False))
+        self.video_streams = check_video_streams(s, self.temporal)
         # NB the reference renders by default (render_mesh is store_false, bev/main.py:44); rendering is out of scope and
         # simply not performed here.
         self.lib = _lib.load()
@@ -228,10 +235,13 @@ class BEV(torch.nn.Module):
         """The video mode (bev/main.py:109-121,260-287): one tracker per instance (shared by every signal_ID), the
         filter sets of MAX_SIGNALS signals, and per slot row buffers for up to 2 x 64 rows per frame."""
         dev, R = self.tdevice, 2 * B * MAX_PERSON
-        self.trk = self.lib.b200romp_bev_tracker_create(self.device_index, TRACKER_MAX_TRACKS, MAX_SIGNALS)
+        if self.video_streams:                         # stream mode: one tracker per signal_ID
+            self.trk = self.lib.b200romp_bev_tracker_create_streams(self.device_index, TRACKER_MAX_TRACKS, self.video_streams)
+        else:
+            self.trk = self.lib.b200romp_bev_tracker_create(self.device_index, TRACKER_MAX_TRACKS, MAX_SIGNALS)
         if not self.trk:
             raise RuntimeError("b200romp_bev_tracker_create: " + self.lib.b200romp_last_error().decode())
-        self.signals = {}                              # signal_ID -> filter set, oldest first (ROMP's TemporalState)
+        self.signals = {}                              # signal_ID -> filter set (stream mode: stream index), oldest first
         z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
         i64, i32 = torch.int64, torch.int32
         self.tshared = dict(det=z(R, dtype=i32), pj2d_org=z(R, 71, 2), keep=z(R, dtype=i32), sel=z(R, dtype=i32))
@@ -252,7 +262,11 @@ class BEV(torch.nn.Module):
 
     def _signal_slots(self, signal_IDs):
         """filter set of every frame's signal_ID; a new signal beyond MAX_SIGNALS evicts the oldest one (its filters are
-        reset on the stream, before the batch's kernel)."""
+        reset on the stream, before the batch's kernel).  Stream mode: the stream index of every frame's signal_ID."""
+        if self.video_streams:
+            return stream_indices(self.signals, signal_IDs, self.video_streams,
+                                  lambda k: _lib.check(self.lib.b200romp_bev_tracker_reset(self.trk, k, C.c_void_p(self.stream.cuda_stream)),
+                                                       "tracker_reset"))
         if len(set(signal_IDs)) > MAX_SIGNALS:
             raise ValueError(f"BEV video mode: at most {MAX_SIGNALS} distinct signal_IDs per batch (their filter sets are "
                              "used by one kernel); split the batch")
@@ -269,10 +283,23 @@ class BEV(torch.nn.Module):
             slots.append(self.signals[sid])
         return slots
 
-    def reset_temporal(self):
-        """Forget every track, id and filter (a new video); ids start again from 1."""
+    def _check_streams(self, signal_IDs):
+        """Stream mode: raise ValueError, before anything is enqueued, when signal_IDs would make more than
+        --video_streams streams live."""
+        if self.video_streams:
+            check_streams(self.signals, [0] if signal_IDs is None else signal_IDs, self.video_streams)
+
+    def reset_temporal(self, signal_ID=None):
+        """Forget every track, id and filter (a new video); ids start again from 1.  Stream mode (--video_streams) with a
+        ``signal_ID``: forget that stream only (its index is freed; when the signal_ID comes back its ids start at 1)."""
         if not self.temporal:
             raise RuntimeError("reset_temporal: this BEV instance was built without -t/--temporal_optimize")
+        if signal_ID is not None:
+            if not self.video_streams:
+                raise ValueError("reset_temporal(signal_ID): only in stream mode (--video_streams); the default mode shares "
+                                 "one tracker across signal_IDs, reset_temporal() forgets it")
+            self.signals.pop(signal_ID, None)          # the index is reset when a signal_ID takes it again
+            return
         _lib.check(self.lib.b200romp_bev_tracker_reset(self.trk, -1, C.c_void_p(self.stream.cuda_stream)), "tracker_reset")
         self.signals = {}
 
@@ -282,6 +309,7 @@ class BEV(torch.nn.Module):
         (b200romp_bev_track_step) between the regressor and SMPL-A, writing the smoothed rows to ``self.tbuf``."""
         b, t, slot = self.buf, self.tbuf, self.slots[self._slot]
         slots = self._signal_slots(signal_IDs)
+        slot["sids"] = list(signal_IDs)
         slot["sig_h2d"].synchronize()                 # the slot's previous chunk has copied its signal slots
         slot["sig_host"][:B].copy_(torch.tensor(slots, dtype=torch.int32))
         t["sig"][:B].copy_(slot["sig_host"][:B], non_blocking=True)
@@ -400,6 +428,11 @@ class BEV(torch.nn.Module):
         if temporal:
             n_rows, n_kept, status = int(h[2]), int(h[3]), int(h[4])
             self.frame_id = int(h[5])
+            if status and self.video_streams:
+                failed = sorted({slot["sids"][b] for b in range(B) if int(h[6 + b]) < 0}, key=repr)
+                raise RuntimeError(f"BEV video mode: more than {TRACKER_MAX_TRACKS} live tracks in the stream(s) of signal_ID "
+                                   f"{', '.join(map(repr, failed))}; call reset_temporal(signal_ID) for each (the other "
+                                   "streams of the batch were tracked)")
             if status:
                 raise RuntimeError("BEV video mode: " + (f"more than {TRACKER_MAX_TRACKS} live tracks" if status == 1 else "too many rows")
                                    + "; call reset_temporal() before the next frame")
@@ -500,6 +533,8 @@ class BEV(torch.nn.Module):
         for every frame, suppressing with ``img_max_side``; or one row per frame ([B,6], numpy or tensor), each frame then
         suppressing with its own max(h, w) (``img_max_side`` is not used).  With -t the frames are consecutive video
         frames, tracked and smoothed in order (``signal_IDs``: one per frame, default 0); the result adds ``track_ids``.
+        With --video_streams every signal_ID is an independent video (its own tracker, ids from 1 and filters,
+        romp_b200/streams.py), stepped in parallel; this holds for every video entry point.
         ``to_numpy=False`` returns device tensors of the caller's current stream (see forward_batches)."""
         sids = None if signal_IDs is None else [signal_IDs]
         return next(self.forward_batches([frames], offsets, center3d_override, to_numpy, img_max_side, sids))
@@ -538,6 +573,7 @@ class BEV(torch.nn.Module):
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         B = frames.shape[0]
+        self._check_streams(signal_IDs)
         slot = self._next_slot()
         fd = frame_buffer(slot["frames"], frames.dtype, B, self.tdevice)
         after_producers(self.copy_stream, self.tdevice, frames)
@@ -594,6 +630,8 @@ class BEV(torch.nn.Module):
                     raise ValueError(f"forward_image_batches: {len(sids)} signal_IDs for {len(imgs)} images")
                 wide = [i for i, t in enumerate(imgs) if self.settings.crowd and t.shape[1] / t.shape[0] >= 2]
                 normal = [i for i in range(len(imgs)) if i not in set(wide)]
+                if self.temporal:
+                    self._check_streams([sids[i] for i in normal])
                 if wide and getattr(self.settings, "show_patch_results", False):
                     raise NotImplementedError("show_patch_results renders and saves per-crop images; rendering is out of scope")
                 if center3d_override is not None:

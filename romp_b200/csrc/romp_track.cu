@@ -4,6 +4,8 @@
 // b200romp_parse and SMPL.  One CTA walks the batch's frames in order, because every frame's association depends on the
 // state the previous frame left; threads parallelise over tracks (argmin, ageing, compaction) and over row channels
 // (smoothing).  The tracker state of every signal and the filter state of every slot stay in device memory.
+// Stream mode (a streams handle): one signal block per stream index, no registration by code; one CTA per stream present
+// in the batch walks that stream's frames with the same per-frame step (romp_track_walk).
 //
 // Per frame with at least one detection (a frame with nobody does nothing, like forward):
 //   signal: a new signal code takes the lowest free block of 64 filter slots and resets all of them; with every block in
@@ -168,9 +170,21 @@ __device__ void rt_age_and_compact(RtSmem& s) {
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kRtThreads) romp_track_kernel(RtDev g, RtIn in, RtOut out) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  RtSmem& s = *reinterpret_cast<RtSmem*>(smem_raw);
+// frames with at least one of the rows [0, n) (grouped by frame); called by every thread of the CTA
+__device__ int rt_frames_with_rows(const long long* batch_ids, int n) {
+  int c = 0;
+  for (int r0 = 0; r0 < n; r0 += blockDim.x) {
+    const int r = r0 + threadIdx.x;
+    c += __syncthreads_count(r < n && (r == 0 || batch_ids[r] != batch_ids[r - 1]));
+  }
+  return c;
+}
+
+// The walk of the batch's frames in order.  stream < 0: every frame, with the signal registration above, and the batch's
+// output count (and the tracked mode's batch ids) written at the end.  stream >= 0 (g offset to that stream's state, one
+// signal block whose code is the stream index): only the frames with sig_code[b] == stream; --show_largest writes frame
+// b's row after the frames before it that have rows.
+__device__ void romp_track_walk(RtSmem& s, const RtDev& g, const RtIn& in, const RtOut& out, int stream) {
   const int tid = threadIdx.x;
   for (int i = tid; i < g.signals * kSigFields; i += blockDim.x) s.sig[i / kSigFields][i % kSigFields] = g.sig[i];
   for (int i = tid; i < g.signals; i += blockDim.x) s.mask[i] = g.mask[i];
@@ -179,6 +193,7 @@ __global__ void __launch_bounds__(kRtThreads) romp_track_kernel(RtDev g, RtIn in
   const int N = min(*in.d_count, in.capacity);
   const bool tracked = !in.show_largest;
   for (int b = 0; b < in.batch; ++b) {
+    if (stream >= 0 && in.sig_code[b] != stream) continue;     // another stream's frame
     if (tid == 0) {                                 // rows of frame b (the parse groups them by frame, in frame order)
       int st = s.st;
       while (st < N && in.batch_ids[st] < b) ++st;
@@ -189,6 +204,10 @@ __global__ void __launch_bounds__(kRtThreads) romp_track_kernel(RtDev g, RtIn in
     __syncthreads();
     const int st = s.st, nf = s.nf;
     if (nf == 0) { __syncthreads(); continue; }     // forward returns before TemporalState.assign
+    if (stream >= 0 && !tracked) {                  // row of frame b = the frames with rows before it
+      const int c = rt_frames_with_rows(in.batch_ids, st);
+      if (tid == 0) s.out0 = c;
+    }
     int fresh = 0;
     if (tid == 0) {                                 // TemporalState.assign: the signal's block
       const int code = in.sig_code[b];
@@ -313,8 +332,35 @@ __global__ void __launch_bounds__(kRtThreads) romp_track_kernel(RtDev g, RtIn in
   if (s.loaded >= 0) rt_table_io(s, g, s.loaded, s.sig[s.loaded][kSigN], false);
   for (int i = tid; i < g.signals * kSigFields; i += blockDim.x) g.sig[i] = s.sig[i / kSigFields][i % kSigFields];
   for (int i = tid; i < g.signals; i += blockDim.x) g.mask[i] = s.mask[i];
+  if (tid == 0) *g.reg = s.reg;
+  if (stream >= 0) return;
   if (tracked) for (int r = tid; r < N; r += blockDim.x) out.batch_ids[r] = in.batch_ids[r];
-  if (tid == 0) { *g.reg = s.reg; *out.d_count = tracked ? N : s.out0; }
+  if (tid == 0) *out.d_count = tracked ? N : s.out0;
+}
+
+__global__ void __launch_bounds__(kRtThreads, 1) romp_track_kernel(RtDev g, RtIn in, RtOut out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  romp_track_walk(*reinterpret_cast<RtSmem*>(smem_raw), g, in, out, -1);
+}
+
+// Stream mode: CTA b steps stream sig_code[b] when frame b is the stream's first frame in the batch; g.signals = streams.
+// CTA 0 also writes the batch's output count (and the tracked mode's batch ids).
+__global__ void __launch_bounds__(kRtThreads, 1) romp_track_streams_kernel(RtDev g, RtIn in, RtOut out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int stream = in.sig_code[blockIdx.x];
+  for (int f = 0; f < (int)blockIdx.x; ++f) if (in.sig_code[f] == stream) return;
+  if (blockIdx.x == 0) {
+    const int N = min(*in.d_count, in.capacity);
+    if (!in.show_largest) for (int r = threadIdx.x; r < N; r += blockDim.x) out.batch_ids[r] = in.batch_ids[r];
+    const int c = in.show_largest ? rt_frames_with_rows(in.batch_ids, N) : N;
+    if (threadIdx.x == 0) *out.d_count = c;
+  }
+  if (stream < 0 || stream >= g.signals) return;      // not a stream of the handle: its frames are left as they are
+  const size_t o = (size_t)stream * kRtTracks, f = (size_t)stream * kRtBlock;
+  g.pt += o * 2; g.id += o; g.age += o; g.slot += o; g.sig += (size_t)stream * kSigFields; g.mask += stream; g.reg += stream;
+  g.oe_raw += f * kOeCh; g.oe_x += f * kOeCh; g.oe_dx += f * kOeCh; g.oe_seen += f;
+  g.signals = 1;
+  romp_track_walk(*reinterpret_cast<RtSmem*>(smem_raw), g, in, out, stream);
 }
 
 constexpr size_t kRtSmem = sizeof(RtSmem);
@@ -325,8 +371,37 @@ using namespace b200romp;
 
 struct b200romp_romp_tracker {
   int device = 0;
+  int streams = 0;     // 0: max_signals signals registered by code; > 0: that many independent streams (stream mode)
   RtDev d{};
 };
+
+static b200romp_romp_tracker* romp_tracker_new(int device, int signals, int streams) {
+  b200romp_romp_tracker* t = new b200romp_romp_tracker();
+  t->device = device;
+  t->streams = streams;
+  RtDev& d = t->d;
+  d.signals = signals;
+  const size_t T = (size_t)signals * kRtTracks, slots = (size_t)signals * kRtBlock, nf = slots * kOeCh * sizeof(float);
+  const size_t regs = streams > 0 ? streams : 1;     // registration counters: one per stream
+  bool ok = cudaMalloc(&d.pt, T * 2 * sizeof(double)) == cudaSuccess && cudaMalloc(&d.id, T * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.age, T * sizeof(int)) == cudaSuccess && cudaMalloc(&d.slot, T * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.sig, signals * kSigFields * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.mask, signals * sizeof(unsigned long long)) == cudaSuccess &&
+            cudaMalloc(&d.reg, regs * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.oe_raw, nf) == cudaSuccess && cudaMalloc(&d.oe_x, nf) == cudaSuccess && cudaMalloc(&d.oe_dx, nf) == cudaSuccess &&
+            cudaMalloc(&d.oe_seen, slots * sizeof(int)) == cudaSuccess &&
+            cudaFuncSetAttribute(romp_track_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRtSmem) == cudaSuccess &&
+            cudaFuncSetAttribute(romp_track_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRtSmem) == cudaSuccess &&
+            cudaMemset(d.sig, 0, signals * kSigFields * sizeof(int)) == cudaSuccess &&
+            cudaMemset(d.mask, 0, signals * sizeof(unsigned long long)) == cudaSuccess &&
+            cudaMemset(d.reg, 0, regs * sizeof(int)) == cudaSuccess && cudaMemset(d.oe_seen, 0, slots * sizeof(int)) == cudaSuccess;
+  if (!ok) {
+    set_error("romp_tracker_create: allocation failed");
+    b200romp_romp_tracker_destroy(t);
+    return nullptr;
+  }
+  return t;
+}
 
 extern "C" {
 
@@ -335,28 +410,15 @@ b200romp_romp_tracker* b200romp_romp_tracker_create(int device, int max_signals)
     set_error("romp_tracker_create: bad arguments (1 <= max_signals <= %d) / no CUDA device", kRtMaxSignals);
     return nullptr;
   }
-  b200romp_romp_tracker* t = new b200romp_romp_tracker();
-  t->device = device;
-  RtDev& d = t->d;
-  d.signals = max_signals;
-  const size_t T = (size_t)max_signals * kRtTracks, slots = (size_t)max_signals * kRtBlock, nf = slots * kOeCh * sizeof(float);
-  bool ok = cudaMalloc(&d.pt, T * 2 * sizeof(double)) == cudaSuccess && cudaMalloc(&d.id, T * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.age, T * sizeof(int)) == cudaSuccess && cudaMalloc(&d.slot, T * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.sig, max_signals * kSigFields * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.mask, max_signals * sizeof(unsigned long long)) == cudaSuccess &&
-            cudaMalloc(&d.reg, sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.oe_raw, nf) == cudaSuccess && cudaMalloc(&d.oe_x, nf) == cudaSuccess && cudaMalloc(&d.oe_dx, nf) == cudaSuccess &&
-            cudaMalloc(&d.oe_seen, slots * sizeof(int)) == cudaSuccess &&
-            cudaFuncSetAttribute(romp_track_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRtSmem) == cudaSuccess &&
-            cudaMemset(d.sig, 0, max_signals * kSigFields * sizeof(int)) == cudaSuccess &&
-            cudaMemset(d.mask, 0, max_signals * sizeof(unsigned long long)) == cudaSuccess &&
-            cudaMemset(d.reg, 0, sizeof(int)) == cudaSuccess && cudaMemset(d.oe_seen, 0, slots * sizeof(int)) == cudaSuccess;
-  if (!ok) {
-    set_error("romp_tracker_create: allocation failed");
-    b200romp_romp_tracker_destroy(t);
+  return romp_tracker_new(device, max_signals, 0);
+}
+
+b200romp_romp_tracker* b200romp_romp_tracker_create_streams(int device, int streams) {
+  if (streams <= 0 || streams > B200ROMP_MAX_VIDEO_STREAMS || cudaSetDevice(device) != cudaSuccess) {
+    set_error("romp_tracker_create_streams: bad arguments (1 <= streams <= %d) / no CUDA device", B200ROMP_MAX_VIDEO_STREAMS);
     return nullptr;
   }
-  return t;
+  return romp_tracker_new(device, streams, streams);
 }
 
 void b200romp_romp_tracker_destroy(b200romp_romp_tracker* t) {
@@ -375,8 +437,19 @@ int b200romp_romp_tracker_reset(b200romp_romp_tracker* t, b200romp_stream stream
   const RtDev& d = t->d;
   B2R_CUDA_OK(cudaMemsetAsync(d.sig, 0, d.signals * kSigFields * sizeof(int), stream));   // every block free
   B2R_CUDA_OK(cudaMemsetAsync(d.mask, 0, d.signals * sizeof(unsigned long long), stream));
-  B2R_CUDA_OK(cudaMemsetAsync(d.reg, 0, sizeof(int), stream));
+  B2R_CUDA_OK(cudaMemsetAsync(d.reg, 0, (t->streams > 0 ? t->streams : 1) * sizeof(int), stream));
   B2R_CUDA_OK(cudaMemsetAsync(d.oe_seen, 0, (size_t)d.signals * kRtBlock * sizeof(int), stream));
+  return B200ROMP_OK;
+}
+
+int b200romp_romp_tracker_reset_stream(b200romp_romp_tracker* t, int s, b200romp_stream stream_) {
+  B2R_REQUIRE(t && t->streams > 0 && s >= 0 && s < t->streams, "romp_tracker_reset_stream: not a stream of a streams handle");
+  B2R_CUDA_OK(cudaSetDevice(t->device));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const RtDev& d = t->d;
+  // a free block: the stream's next frame with rows registers it afresh (no tracks, ids from 1, every filter slot reset)
+  B2R_CUDA_OK(cudaMemsetAsync(d.sig + (size_t)s * kSigFields, 0, kSigFields * sizeof(int), stream));
+  B2R_CUDA_OK(cudaMemsetAsync(d.mask + s, 0, sizeof(unsigned long long), stream));
   return B200ROMP_OK;
 }
 
@@ -390,7 +463,10 @@ int b200romp_romp_track_step(b200romp_romp_tracker* t, int batch, int capacity, 
   B2R_CUDA_OK(cudaSetDevice(t->device));
   RtIn in{d_count, batch_ids, cam, thetas, betas, signal_code, batch, capacity, show_largest, smooth_coeff, freq};
   RtOut out{d_out_count, out_batch_ids, out_thetas, out_betas, out_cam, out_slot, out_track_ids};
-  romp_track_kernel<<<1, kRtThreads, kRtSmem, (cudaStream_t)stream_>>>(t->d, in, out);
+  if (t->streams > 0)
+    romp_track_streams_kernel<<<batch, kRtThreads, kRtSmem, (cudaStream_t)stream_>>>(t->d, in, out);
+  else
+    romp_track_kernel<<<1, kRtThreads, kRtSmem, (cudaStream_t)stream_>>>(t->d, in, out);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
 }

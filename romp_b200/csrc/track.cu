@@ -3,6 +3,9 @@
 // per-(signal, track) One-Euro filters and cam_trans from the smoothed cam, as one kernel per batch placed between
 // the BEV regressor and SMPL-A.  One CTA steps the instance's tracker through the batch's frames in batch order;
 // threads parallelise over tracks, detections, row channels.  Tracker state is fp64 and stays in device memory.
+// Stream mode (a streams handle): one tracker per stream, one CTA per stream present in the batch, each walking its
+// stream's frames with the same per-frame step (bev_track_walk); the rows land in per-frame windows and one more small
+// kernel compacts them in frame order.
 //
 // Per frame with at least one detection (bev/main.py:159-166; a frame with nobody does not step the tracker):
 //   tracking points [(cam2+1)*128, (cam1+1)*128, cam_trans2*30, cam0*128/2] in fp32 (:269-272), scores against 0.12 /
@@ -165,10 +168,11 @@ struct TrkOut {
   int* status;
 };
 
-__global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn in, TrkOut out) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  TrkSmem& s = *reinterpret_cast<TrkSmem*>(smem_raw);
-  double* cost = reinterpret_cast<double*>(smem_raw + ((sizeof(TrkSmem) + 15) / 16) * 16);
+// The walk of one tracker through the batch's frames in order.  stream < 0: the instance's tracker, every frame, filter set
+// sig_slot[b], rows appended in frame order, the batch's counts and status written at the end.  stream >= 0 (g offset to
+// that stream's state, one filter set): only the frames with sig_slot[b] == stream, frame b's rows written to its window
+// [b * 2 * kTrkDet, +nout) for bev_track_compact_kernel; a failed stream marks its frames status[2 + b] = -status.
+__device__ void bev_track_walk(TrkSmem& s, double* cost, const TrkDev& g, const TrkIn& in, const TrkOut& out, int stream) {
   const int tid = threadIdx.x, T = g.T;
   for (int i = tid; i < T * 8; i += blockDim.x) s.mean[i / 8][i % 8] = g.mean[i];
   for (int i = tid; i < T * 3; i += blockDim.x) s.S[i / 3][i % 3] = g.S[i];
@@ -177,17 +181,20 @@ __global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn 
   for (int i = tid; i < kTrkMax; i += blockDim.x) s.upd[i] = -1;
   if (tid < kCtlN) s.ctl[tid] = g.ctl[tid];
   if (tid == 0) { s.st = 0; s.out0 = 0; }
-  for (int b = tid; b < in.batch; b += blockDim.x) out.status[2 + b] = 0;     // rows per frame
+  for (int b = tid; b < in.batch; b += blockDim.x)    // rows per frame
+    if (stream < 0 || in.sig_slot[b] == stream) out.status[2 + b] = 0;
   __syncthreads();
   const int N = min(*in.d_count, in.capacity);
-  for (int b = 0; b < in.batch; ++b) {
+  int b = 0;
+  for (; b < in.batch; ++b) {
     if (s.ctl[kCtlBroken]) break;
+    if (stream >= 0 && in.sig_slot[b] != stream) continue;    // another stream's frame
     if (tid == 0) {                                     // rows of frame b (grouped by frame, in frame order)
       int st = s.st;
       while (st < N && in.batch_ids[st] < b) ++st;
       int e = st;
       while (e < N && in.batch_ids[e] == b) ++e;
-      s.st = st; s.nf = min(e - st, kTrkDet); s.sig = in.sig_slot[b];
+      s.st = st; s.nf = min(e - st, kTrkDet); s.sig = stream < 0 ? in.sig_slot[b] : 0;
     }
     __syncthreads();
     const int st = s.st, nf = s.nf;
@@ -359,6 +366,7 @@ __global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn 
       }
     }
     __syncthreads();
+    if (tid == 0 && stream >= 0) s.out0 = b * 2 * kTrkDet;        // the frame's window
     if (tid == 0 && s.out0 + s.nout > out.capacity) s.ctl[kCtlBroken] = 2;
     __syncthreads();
     if (s.ctl[kCtlBroken]) break;
@@ -414,11 +422,73 @@ __global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn 
   for (int i = tid; i < T * kMetaN; i += blockDim.x) g.meta[i] = s.meta[i / kMetaN][i % kMetaN];
   for (int i = tid; i < T; i += blockDim.x) { g.lists[i] = s.tracked[i]; g.lists[T + i] = s.lost[i]; }
   if (tid < kCtlN) g.ctl[tid] = s.ctl[tid];
-  if (tid == 0) {
+  if (stream >= 0) {                                    // the failed frame and every later frame of the stream
+    if (s.ctl[kCtlBroken])
+      for (int f = b + tid; f < in.batch; f += blockDim.x) if (in.sig_slot[f] == stream) out.status[2 + f] = -s.ctl[kCtlBroken];
+  } else if (tid == 0) {
     *out.d_count = s.out0;
     out.status[0] = s.ctl[kCtlBroken];
     out.status[1] = s.ctl[kCtlFrame];
   }
+}
+
+__global__ void __launch_bounds__(kTrkThreads) bev_track_kernel(TrkDev g, TrkIn in, TrkOut out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  TrkSmem& s = *reinterpret_cast<TrkSmem*>(smem_raw);
+  double* cost = reinterpret_cast<double*>(smem_raw + ((sizeof(TrkSmem) + 15) / 16) * 16);
+  bev_track_walk(s, cost, g, in, out, -1);
+}
+
+// Stream mode: CTA b steps stream sig_slot[b] when frame b is the stream's first frame in the batch; g.signals = streams.
+__global__ void __launch_bounds__(kTrkThreads) bev_track_streams_kernel(TrkDev g, TrkIn in, TrkOut out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  TrkSmem& s = *reinterpret_cast<TrkSmem*>(smem_raw);
+  double* cost = reinterpret_cast<double*>(smem_raw + ((sizeof(TrkSmem) + 15) / 16) * 16);
+  const int stream = in.sig_slot[blockIdx.x], T = g.T;
+  for (int f = 0; f < (int)blockIdx.x; ++f) if (in.sig_slot[f] == stream) return;
+  if (stream < 0 || stream >= g.signals) {              // not a stream of the handle: its frames fail
+    for (int f = threadIdx.x; f < in.batch; f += blockDim.x) if (in.sig_slot[f] == stream) out.status[2 + f] = -3;
+    return;
+  }
+  const size_t o = (size_t)stream * T;
+  g.mean += o * 8; g.S += o * 3; g.meta += o * kMetaN; g.lists += o * 2; g.ctl += (size_t)stream * kCtlN;
+  g.oe_raw += o * kOeCh; g.oe_x += o * kOeCh; g.oe_dx += o * kOeCh; g.oe_seen += o;
+  g.signals = 1;
+  bev_track_walk(s, cost, g, in, out, stream);
+}
+
+// Stream mode, after bev_track_streams_kernel (one CTA): moves every frame's rows from its window to the end of the
+// previous frames' rows, in frame order.  A frame's rows move down by d = window start - destination; copying them in
+// chunks of at most d rows never overwrites a row before it is read.  Writes *d_count and status[0] = the frames whose
+// stream failed, status[1] = 0.
+template <typename V>
+__device__ __forceinline__ void trk_move_rows(V* p, int w, int dst, int src, int n) {
+  for (int e = threadIdx.x; e < n * w; e += blockDim.x) p[(size_t)dst * w + e] = p[(size_t)src * w + e];
+}
+
+__global__ void __launch_bounds__(1024) bev_track_compact_kernel(TrkOut out, int batch) {
+  int total = 0, failed = 0;
+  for (int b = 0; b < batch; ++b) {
+    const int n = out.status[2 + b], src = b * 2 * kTrkDet;
+    failed += n < 0;
+    if (n <= 0) continue;
+    const int d = src - total;
+    for (int r0 = 0; r0 < n && d > 0; r0 += d) {
+      const int c = min(d, n - r0), from = src + r0, to = total + r0;
+      trk_move_rows(out.batch_ids, 1, to, from, c);
+      trk_move_rows(out.track_ids, 1, to, from, c);
+      trk_move_rows(out.det, 1, to, from, c);
+      trk_move_rows(out.conf, 1, to, from, c);
+      trk_move_rows(out.thetas, 72, to, from, c);
+      trk_move_rows(out.betas, 11, to, from, c);
+      trk_move_rows(out.cam, 3, to, from, c);
+      trk_move_rows(out.cam_trans, 3, to, from, c);
+      trk_move_rows(out.params, 146, to, from, c);
+      __syncthreads();
+    }
+    total += n;
+  }
+  if (threadIdx.x == 0) { *out.d_count = total; out.status[0] = failed; out.status[1] = 0; }
 }
 
 constexpr size_t kTrkSmem = ((sizeof(TrkSmem) + 15) / 16) * 16 + sizeof(double) * kTrkMax * kTrkDet;
@@ -429,8 +499,40 @@ using namespace b200romp;
 
 struct b200romp_bev_tracker {
   int device = 0;
+  int streams = 0;     // 0: one tracker and max_signals filter sets; > 0: that many independent trackers (stream mode)
   TrkDev d{};
 };
+
+static b200romp_bev_tracker* bev_tracker_new(int device, int max_tracks, int filter_sets, int streams) {
+  b200romp_bev_tracker* t = new b200romp_bev_tracker();
+  t->device = device;
+  t->streams = streams;
+  TrkDev& d = t->d;
+  d.T = max_tracks; d.signals = filter_sets;
+  const size_t trackers = streams > 0 ? streams : 1, T = trackers * max_tracks;
+  const size_t slots = (size_t)filter_sets * max_tracks, nf = slots * kOeCh * sizeof(float);
+  bool ok = cudaMalloc(&d.mean, T * 8 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&d.S, T * 3 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&d.meta, T * kMetaN * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.lists, 2 * T * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.ctl, trackers * kCtlN * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&d.oe_raw, nf) == cudaSuccess && cudaMalloc(&d.oe_x, nf) == cudaSuccess && cudaMalloc(&d.oe_dx, nf) == cudaSuccess &&
+            cudaMalloc(&d.oe_seen, slots * sizeof(int)) == cudaSuccess &&
+            cudaFuncSetAttribute(bev_track_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrkSmem) == cudaSuccess &&
+            cudaFuncSetAttribute(bev_track_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrkSmem) == cudaSuccess &&
+            cudaMemset(d.mean, 0, T * 8 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(d.S, 0, T * 3 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(d.meta, 0, T * kMetaN * sizeof(int)) == cudaSuccess &&
+            cudaMemset(d.lists, 0, 2 * T * sizeof(int)) == cudaSuccess &&
+            cudaMemset(d.ctl, 0, trackers * kCtlN * sizeof(int)) == cudaSuccess &&
+            cudaMemset(d.oe_seen, 0, slots * sizeof(int)) == cudaSuccess;
+  if (!ok) {
+    set_error("bev_tracker_create: allocation failed");
+    b200romp_bev_tracker_destroy(t);
+    return nullptr;
+  }
+  return t;
+}
 
 extern "C" {
 
@@ -439,29 +541,17 @@ b200romp_bev_tracker* b200romp_bev_tracker_create(int device, int max_tracks, in
     set_error("bev_tracker_create: bad arguments (1 <= max_tracks <= %d, max_signals >= 1) / no CUDA device", kTrkMax);
     return nullptr;
   }
-  b200romp_bev_tracker* t = new b200romp_bev_tracker();
-  t->device = device;
-  TrkDev& d = t->d;
-  d.T = max_tracks; d.signals = max_signals;
-  const size_t slots = (size_t)max_signals * max_tracks, nf = slots * kOeCh * sizeof(float);
-  bool ok = cudaMalloc(&d.mean, max_tracks * 8 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&d.S, max_tracks * 3 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&d.meta, max_tracks * kMetaN * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.lists, 2 * max_tracks * sizeof(int)) == cudaSuccess && cudaMalloc(&d.ctl, kCtlN * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d.oe_raw, nf) == cudaSuccess && cudaMalloc(&d.oe_x, nf) == cudaSuccess && cudaMalloc(&d.oe_dx, nf) == cudaSuccess &&
-            cudaMalloc(&d.oe_seen, slots * sizeof(int)) == cudaSuccess &&
-            cudaFuncSetAttribute(bev_track_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrkSmem) == cudaSuccess &&
-            cudaMemset(d.mean, 0, max_tracks * 8 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(d.S, 0, max_tracks * 3 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(d.meta, 0, max_tracks * kMetaN * sizeof(int)) == cudaSuccess &&
-            cudaMemset(d.lists, 0, 2 * max_tracks * sizeof(int)) == cudaSuccess && cudaMemset(d.ctl, 0, kCtlN * sizeof(int)) == cudaSuccess &&
-            cudaMemset(d.oe_seen, 0, slots * sizeof(int)) == cudaSuccess;
-  if (!ok) {
-    set_error("bev_tracker_create: allocation failed");
-    b200romp_bev_tracker_destroy(t);
+  return bev_tracker_new(device, max_tracks, max_signals, 0);
+}
+
+b200romp_bev_tracker* b200romp_bev_tracker_create_streams(int device, int max_tracks, int streams) {
+  if (max_tracks <= 0 || max_tracks > kTrkMax || streams <= 0 || streams > B200ROMP_MAX_VIDEO_STREAMS ||
+      cudaSetDevice(device) != cudaSuccess) {
+    set_error("bev_tracker_create_streams: bad arguments (1 <= max_tracks <= %d, 1 <= streams <= %d) / no CUDA device", kTrkMax,
+              B200ROMP_MAX_VIDEO_STREAMS);
     return nullptr;
   }
-  return t;
+  return bev_tracker_new(device, max_tracks, streams, streams);
 }
 
 void b200romp_bev_tracker_destroy(b200romp_bev_tracker* t) {
@@ -479,10 +569,15 @@ int b200romp_bev_tracker_reset(b200romp_bev_tracker* t, int signal, b200romp_str
   cudaStream_t stream = (cudaStream_t)stream_;
   const TrkDev& d = t->d;
   if (signal < 0) {
-    B2R_CUDA_OK(cudaMemsetAsync(d.meta, 0, d.T * kMetaN * sizeof(int), stream));
-    B2R_CUDA_OK(cudaMemsetAsync(d.ctl, 0, kCtlN * sizeof(int), stream));
+    const size_t trackers = t->streams > 0 ? t->streams : 1;
+    B2R_CUDA_OK(cudaMemsetAsync(d.meta, 0, trackers * d.T * kMetaN * sizeof(int), stream));
+    B2R_CUDA_OK(cudaMemsetAsync(d.ctl, 0, trackers * kCtlN * sizeof(int), stream));
     B2R_CUDA_OK(cudaMemsetAsync(d.oe_seen, 0, (size_t)d.signals * d.T * sizeof(int), stream));
   } else {
+    if (t->streams > 0) {                              // the stream's tracker: no tracks, frame_id 0, ids from 1
+      B2R_CUDA_OK(cudaMemsetAsync(d.meta + (size_t)signal * d.T * kMetaN, 0, d.T * kMetaN * sizeof(int), stream));
+      B2R_CUDA_OK(cudaMemsetAsync(d.ctl + (size_t)signal * kCtlN, 0, kCtlN * sizeof(int), stream));
+    }
     B2R_CUDA_OK(cudaMemsetAsync(d.oe_seen + (size_t)signal * d.T, 0, d.T * sizeof(int), stream));
   }
   return B200ROMP_OK;
@@ -502,7 +597,13 @@ int b200romp_bev_track_step(b200romp_bev_tracker* t, int batch, int capacity, co
   TrkIn in{d_count, batch_ids, conf, cam, cam_trans, thetas, betas, params_pred, signal_slot, batch, capacity, show_largest, smooth_coeff};
   TrkOut out{out_capacity, d_out_count, out_batch_ids, out_track_ids, out_det, out_thetas, out_betas, out_cam, out_cam_trans,
              out_params_pred, out_conf, d_status};
-  bev_track_kernel<<<1, kTrkThreads, kTrkSmem, (cudaStream_t)stream_>>>(t->d, in, out);
+  if (t->streams > 0) {
+    bev_track_streams_kernel<<<batch, kTrkThreads, kTrkSmem, (cudaStream_t)stream_>>>(t->d, in, out);
+    B2R_CUDA_OK(cudaGetLastError());
+    bev_track_compact_kernel<<<1, 1024, 0, (cudaStream_t)stream_>>>(out, batch);
+  } else {
+    bev_track_kernel<<<1, kTrkThreads, kTrkSmem, (cudaStream_t)stream_>>>(t->d, in, out);
+  }
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
 }

@@ -22,6 +22,7 @@ import torch
 
 from . import _lib, graph
 from ._lib import BF16, F32, U8
+from .streams import MAX_VIDEO_STREAMS, check_video_streams, stream_indices
 from .staging import (FULL_FRAME, RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch,
                       split_by_frame, to_caller)
 
@@ -66,6 +67,10 @@ def romp_settings(input_args=sys.argv[1:]):
                              "utils.py:347-389); pnp = the reference's default cv2.solvePnPRansac per person on the host; "
                              "epnp = the reference's RANSAC loop and validity mask on the GPU, with the published EPnP as "
                              "its solver (every entry point)")
+    parser.add_argument("--video_streams", type=int, default=0,
+                        help=f"with -t: track up to N independent videos (one per signal_ID, each with its own tracker, ids "
+                             f"and filters), stepped in parallel on the GPU by forward_video(_batches) and forward; 0 = the "
+                             f"per-instance signal table (at most {MAX_VIDEO_STREAMS})")
     args = parser.parse_args(input_args)
     if not os.path.exists(args.smpl_path):
         alt = args.smpl_path.replace("SMPL_NEUTRAL.pth", "smpl_packed_info.pth")   # main.py:50-52
@@ -212,6 +217,7 @@ class ROMP(torch.nn.Module):
                                       "seam the reference swaps for its ONNX session (main.py:78-91,108-110)")
         if getattr(s, "show_largest", False) and not getattr(s, "temporal_optimize", False):
             raise NotImplementedError("--show_largest only selects the smoothed person of --temporal_optimize (main.py:128-134)")
+        self.video_streams = check_video_streams(s, bool(getattr(s, "temporal_optimize", False)))
         self.lib = _lib.load()
         self.device_index = int(s.GPU)
         self.tdevice = torch.device("cuda", self.device_index)
@@ -239,11 +245,15 @@ class ROMP(torch.nn.Module):
                 raise RuntimeError("b200romp_tracks_create: " + self.lib.b200romp_last_error().decode())
             self._slot_host = torch.zeros(self.cap, dtype=torch.int32).pin_memory()
             self._slot_dev = torch.zeros(self.cap, dtype=torch.int32, device=self.tdevice)
-            # forward_video's device tracker: its own signals, tracks and filters (csrc/romp_track.cu)
-            self._rtrack = self.lib.b200romp_romp_tracker_create(self.device_index, self.temporal.max_signals)
+            # forward_video's device tracker: its own signals, tracks and filters (csrc/romp_track.cu); stream mode: one
+            # independent tracker per signal_ID, which forward shares
+            if self.video_streams:
+                self._rtrack = self.lib.b200romp_romp_tracker_create_streams(self.device_index, self.video_streams)
+            else:
+                self._rtrack = self.lib.b200romp_romp_tracker_create(self.device_index, self.temporal.max_signals)
             if not self._rtrack:
                 raise RuntimeError("b200romp_romp_tracker_create: " + self.lib.b200romp_last_error().decode())
-            self._signal_codes = {}          # signal_ID -> int32 code of the device tracker
+            self._signal_codes = {}          # signal_ID -> int32 code of the device tracker (stream mode: stream index)
             self._temporal_user = None       # "forward" / "video": which path holds the tracker state
 
     # ------------------------------------------------------------------------------------------
@@ -604,6 +614,11 @@ class ROMP(torch.nn.Module):
     def forward(self, image, signal_ID=0, **kwargs):
         """image: HxWx3 uint8 BGR (cv2.imread).  main.py:160-176; preprocessing, model, parse, SMPL and projection all run
         on the GPU - OpenCV is not involved."""
+        if self.temporal is not None and self.video_streams:     # stream mode: one state for forward and forward_video
+            out = self.forward_video([image], [signal_ID])[0]
+            if out is None:
+                print("None person detected")
+            return out
         if self.temporal is not None:
             self._claim_temporal("forward")
             return self._forward_temporal(image, signal_ID)
@@ -673,11 +688,17 @@ class ROMP(torch.nn.Module):
                                f"reset_temporal() before switching to {user}()")
         self._temporal_user = user
 
-    def reset_temporal(self):
+    def reset_temporal(self, signal_ID=None):
         """Start a new video: forget every signal, track id and filter of both forward() and forward_video(); ids count
-        from 1 again."""
+        from 1 again.  Stream mode (--video_streams) with a ``signal_ID``: forget that stream only (its index is freed;
+        when the signal_ID comes back its ids start at 1)."""
         if self.temporal is None:
             raise RuntimeError("reset_temporal: this ROMP instance was built without -t/--temporal_optimize")
+        if signal_ID is not None:
+            if not self.video_streams:
+                raise ValueError("reset_temporal(signal_ID): only in stream mode (--video_streams)")
+            self._signal_codes.pop(signal_ID, None)    # the index is reset when a signal_ID takes it again
+            return
         from .temporal import TemporalState
         sp = C.c_void_p(self.stream.cuda_stream)
         self.temporal = TemporalState(self.temporal.show_largest, self.temporal.max_signals)
@@ -685,6 +706,11 @@ class ROMP(torch.nn.Module):
         _lib.check(self.lib.b200romp_romp_tracker_reset(self._rtrack, sp), "romp_tracker_reset")
         self._signal_codes = {}
         self._temporal_user = None
+
+    def _reset_stream(self, k):
+        """Stream mode: stream index k starts afresh, on the model's stream (before the next track step)."""
+        _lib.check(self.lib.b200romp_romp_tracker_reset_stream(self._rtrack, k, C.c_void_p(self.stream.cuda_stream)),
+                   "romp_tracker_reset_stream")
 
     def _video_buffers(self, slot):
         """The track step's outputs of one slot (allocated on first use): the smoothed rows SMPL runs on, the per-row
@@ -789,7 +815,8 @@ class ROMP(torch.nn.Module):
         signal_IDs[i])`` returns in a loop on a fresh instance, or None; nothing is printed.  Like forward's temporal path
         it keeps the device's cam_trans: the closed form, or ``--cam_trans epnp`` on the smoothed rows (``--cam_trans pnp``,
         a host step, is not applied).  center_override: optional device
-        [n,1,64,64] replacing the images' center maps (tests, measurement)."""
+        [n,1,64,64] replacing the images' center maps (tests, measurement).  With --video_streams every signal_ID is an
+        independent video (its own tracker, ids from 1 and filters, romp_b200/streams.py), stepped in parallel."""
         sids = None if signal_IDs is None else [signal_IDs]
         return next(self.forward_video_batches([images], sids, to_numpy, center_override))
 
@@ -812,7 +839,10 @@ class ROMP(torch.nn.Module):
                 if len(sids) != len(imgs):
                     raise ValueError(f"forward_video: {len(sids)} signal_IDs for {len(imgs)} images")
                 self._claim_temporal("video")
-                codes = [self._signal_codes.setdefault(sid, len(self._signal_codes)) for sid in sids]
+                if self.video_streams:
+                    codes = stream_indices(self._signal_codes, sids, self.video_streams, self._reset_stream)
+                else:
+                    codes = [self._signal_codes.setdefault(sid, len(self._signal_codes)) for sid in sids]
                 res = [None] * len(imgs)
                 if not imgs:
                     yield res, imgs, codes, 0, True
