@@ -284,6 +284,32 @@ long long b200romp_bev_long_merge_workspace_bytes(int capacity);
 int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
                             const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
                             float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream);
+/* Crowd mode for several wide images at once (bev/main.py:139-143,184-258 for each image): b200romp_bev_crop_post for a
+ * chunk whose crops may belong to several images.  crop_table and crop0 index the pass's crops, every image's crops in
+ * order; crop_images: DEVICE int32 [n_crops][2] = {image, first accumulation row of that image} per crop.  Each crop's
+ * survivors are appended at its own image's running count: image j's rows start at its first row, acc_count[2j] counts
+ * them and acc_count[2j+1] the persons detected in its crops (zero acc_count[0, 2n) before a pass); within an image the
+ * rows come in crop order, then in score order.  acc_capacity bounds all the rows; acc_ctl [2*batch] is scratch.
+ * b200romp_bev_crop_post is the one-image case. */
+int b200romp_bev_crop_post_images(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                                  const float* thetas, const float* params_pred, const float* conf, const float* cam,
+                                  const float* cam_trans, const long long* batch_ids, int batch, int capacity, const int* d_count,
+                                  const float* crop_table, const int* crop_images, int crop0, float rel_scale_thresh, float* pj2d,
+                                  int* keep, int* sel, float* cam_full, int acc_capacity, int* acc_count, int* acc_ctl,
+                                  float* acc_verts, float* acc_joints, float* acc_thetas, float* acc_betas, float* acc_params_pred,
+                                  float* acc_conf, float* acc_cam, b200romp_stream stream);
+/* b200romp_bev_long_merge for n_images images in one launch sequence (bev/main.py:253-256 for each image): image j has
+ * acc_count[2j] accumulated rows from row row_base[j] (DEVICE int32 [n_images], ascending; at most image_rows rows per
+ * image), projects with its row of the DEVICE fp32 pad_table [n_images,6] and suppresses with (float)(nms_thresh *
+ * max(h,w,3) / 640) of that row.  The kept rows of all images go to sel in image order, img_sel [n_images][2] =
+ * {start in sel, count} per image (DEVICE int32), *d_count_out = their total, so b200romp_gather_rows copies a field of
+ * every image in one call.  removed [capacity], workspace of b200romp_bev_long_merge_images_workspace_bytes(capacity,
+ * n_images) bytes.  b200romp_bev_long_merge is the one-image case (its workspace holds the same values). */
+long long b200romp_bev_long_merge_images_workspace_bytes(int capacity, int n_images);
+int b200romp_bev_long_merge_images(const float* cam, const float* joints, const float* conf, int capacity, int n_images,
+                                   int image_rows, const int* row_base, const int* acc_count, const float* pad_table, double nms_thresh,
+                                   float rel_scale_thresh, float* cam_trans, float* pj2d_org, int* removed, void* workspace, int* sel,
+                                   int* img_sel, int* d_count_out, b200romp_stream stream);
 /* dst[i] = src[sel[i]] for i < *d_count; rows of row_bytes (multiple of 4) bytes. */
 int b200romp_gather_rows(const void* src, int row_bytes, const int* sel, const int* d_count, int capacity, void* dst,
                          b200romp_stream stream);

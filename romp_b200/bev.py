@@ -4,7 +4,7 @@
 True and therefore overrides the thresholds with ``long_conf_dict``), ``BEV(settings)(image_bgr) -> dict | None``
 mirrors bev/main.py:91-258: normal images run as one 512x512 frame, and in crowd mode images at least twice as wide as
 high run through ``process_long_image`` (the reference's overlapping crops, batched through the model, with the per-crop
-and merged filters on the device).  ``forward_batch`` is the batched entry point for normal frames, ``forward_images`` the
+and merged filters on the device; ``process_long_images`` for a list of them, in passes of several images).  ``forward_batch`` is the batched entry point for normal frames, ``forward_images`` the
 batched ``forward`` on raw images of different sizes (each frame with its own geometry); ``forward_batches`` and
 ``forward_image_batches`` stream them on two slots, staging and reading back neighbouring chunks while a chunk's kernels run.
 Per-frame semantics of the two post filters (bev/post_parser.py:167-222) are preserved by applying them per
@@ -104,6 +104,31 @@ def long_image_plan(h, w, overlap_ratio):
         boxes.append([left, right, 0, h])
     top = (w - h) // 2
     return pad_length, np.array(boxes).astype(np.int32), np.array([top, w - top, 0, w, h, w], np.float32)
+
+
+def long_images_plan(shapes, overlap_ratio, max_crops):
+    """``long_image_plan`` of every (h, w) in ``shapes``, concatenated in list order, and the list cut into passes.
+
+    Returns a dict: boxes int32 [K,4] (every image's boxes in order: the global crop sequence), image int64 [K] (the image
+    of each crop), first_crop int64 [n+1] (image j's crops are first_crop[j] .. first_crop[j+1]-1), row_base int64 [n] (64
+    x its first crop: where its accumulated rows start), pad_length [n], pad_info fp32 [n,6], img_max_side [n] (max(h, w))
+    and passes [(i0, i1)]: images i0 .. i1-1, whole images in list order while their crops total at most
+    max(max_crops, K of the pass's first image), so an image with more crops than max_crops is a pass of its own."""
+    plans = [long_image_plan(h, w, overlap_ratio) for h, w in shapes]
+    counts = [len(p[1]) for p in plans]
+    first = np.cumsum([0] + counts)
+    passes, i0 = [], 0
+    while i0 < len(shapes):
+        i1, total = i0 + 1, counts[i0]
+        while i1 < len(shapes) and total + counts[i1] <= max(max_crops, counts[i0]):
+            total += counts[i1]
+            i1 += 1
+        passes.append((i0, i1))
+        i0 = i1
+    return dict(boxes=np.concatenate([p[1] for p in plans]).astype(np.int32) if plans else np.zeros((0, 4), np.int32),
+                image=np.repeat(np.arange(len(shapes)), counts), first_crop=first, row_base=MAX_PERSON * first[:-1],
+                pad_length=[p[0] for p in plans], pad_info=np.array([p[2] for p in plans], np.float32).reshape(-1, 6),
+                img_max_side=[max(h, w) for h, w in shapes], passes=passes)
 
 
 def long_image_crop_table(boxes, pad_length, h, w, nms_thresh):
@@ -209,7 +234,6 @@ class BEV(torch.nn.Module):
         self._slot = 0
         self.copy_stream = torch.cuda.Stream(device=dev)
         self.d2h_stream = torch.cuda.Stream(device=dev)
-        self.count_host = torch.zeros(2, dtype=torch.int32).pin_memory()      # the long-image mode's read-back
 
     @property
     def buf(self):
@@ -389,14 +413,6 @@ class BEV(torch.nn.Module):
             src = b["conf"] if k == "conf" else b[k]
             row = src[0].numel() * src.element_size()
             _lib.check(lib.b200romp_gather_rows(_ptr(src), row, _ptr(b["sel"]), _ptr(b["count2"]), cap, _ptr(dst), sp), "gather_rows")
-
-    def _counts(self, detected, kept):
-        """The host sync of a long-image result: (persons detected, persons kept by the filters) from two device counters."""
-        with torch.cuda.stream(self.stream):
-            self.count_host[0:1].copy_(detected, non_blocking=True)
-            self.count_host[1:2].copy_(kept, non_blocking=True)
-        self.stream.synchronize()
-        return int(self.count_host[0]), int(self.count_host[1])
 
     def _result(self, src, n, batch_ids):
         """The output dict (result_keys, plus the SMPL outputs): device views of the first n rows of the buffers ``src``."""
@@ -596,7 +612,7 @@ class BEV(torch.nn.Module):
         not the host OpenCV resize of ``forward``) and b200romp_bev_post_frames, each frame with its own pad info and
         suppression threshold; element i then equals ``forward_batch`` on image i's GPU-preprocessed frame with its pad
         info and ``img_max_side = max(h, w)``.  A frame with a detection whose persons were all filtered out gives a dict
-        of empty arrays.  In crowd mode images with w/h >= 2 go one by one through ``process_long_image``.
+        of empty arrays.  In crowd mode the images with w/h >= 2 go together through ``process_long_images``.
         center3d_override: optional device [n_normal,64,128,128] for the normal images in order.
         With -t the normal images are consecutive video frames (``signal_IDs``: one per image, default 0), tracked and
         smoothed in list order; wide crowd-mode images are neither tracked nor smoothed (bev/main.py:140-143)."""
@@ -609,7 +625,8 @@ class BEV(torch.nn.Module):
         ``forward_images`` returns for it, in order.  Each chunk of at most ``max_batch`` normal images is staged into
         its slot's pinned buffer and sent with one H2D on the copy stream (device images are read in place), so staging
         chunk i+1 and reading back chunk i-1 overlap the kernels of chunk i (the two slots of ``forward_batches``).  A
-        wide crowd-mode image drains the pipeline and runs through ``process_long_image`` between its list's chunks.
+        list's wide crowd-mode images drain the pipeline once and run through one ``process_long_images`` call (one host
+        sync per pass) before the list's first chunk.
         center3d_override applies to every list, entry k to the k-th normal image of the list.  With -t the lists are
         consecutive parts of one video (tracker and filters carry across them) and ``signal_IDs`` is None or one sequence
         per list.  Host images have been staged when the generator pulls the next list; device images and
@@ -622,7 +639,7 @@ class BEV(torch.nn.Module):
 
         def chunks():
             """(images, signal IDs, result list, the chunk's normal images, their 3-D centre maps, the wide images to run
-            before the chunk, last chunk of the list)"""
+            before the chunk (all of the list's, before its first chunk), last chunk of the list)"""
             for images in batches:
                 imgs = [image_tensor(x) for x in images]
                 sids = [0] * len(imgs) if sid_iter is None else list(next(sid_iter))
@@ -640,10 +657,8 @@ class BEV(torch.nn.Module):
                 for c0 in range(0, max(len(normal), 1), self.max_batch):
                     idx = normal[c0:c0 + self.max_batch]
                     last = c0 + self.max_batch >= len(normal)
-                    now = [i for i in wide if last or i < idx[0]]
-                    wide = wide[len(now):]
                     co = None if center3d_override is None or not idx else center3d_override[c0:c0 + len(idx)]
-                    yield imgs, sids, res, idx, co, now, last
+                    yield imgs, sids, res, idx, co, wide if c0 == 0 else [], last
 
         pending = None
         for imgs, sids, res, idx, co, wide, last in chunks():
@@ -652,8 +667,9 @@ class BEV(torch.nn.Module):
                 pending = None
                 if done is not None:
                     yield done
-            for i in wide:
-                res[i] = self.process_long_image(imgs[i], to_numpy=to_numpy)
+            if wide:
+                for i, r in zip(wide, self.process_long_images([imgs[i] for i in wide], to_numpy=to_numpy)):
+                    res[i] = r
             slot = self._submit_images([imgs[i] for i in idx], co, [sids[i] for i in idx]) if idx else None
             if pending is not None:
                 done = self._finish_images(*pending, to_numpy)
@@ -690,18 +706,23 @@ class BEV(torch.nn.Module):
                 res[i] = r
         return res if last else None
 
-    def _long_buffers(self, rows):
-        """Image-level accumulation rows of the long-image mode (grown on demand, kept for the next image)."""
+    def _long_buffers(self, rows, n_images=1):
+        """Accumulation rows of the long-image mode for a pass of up to n_images images (grown on demand, kept for the
+        next pass)."""
         lb = getattr(self, "_long", None)
-        if lb is not None and lb["cam"].shape[0] >= rows:
+        if lb is not None and lb["cam"].shape[0] >= rows and lb["img_sel"].shape[0] >= n_images:
             return lb
+        if lb is not None:
+            rows, n_images = max(rows, lb["cam"].shape[0]), max(n_images, lb["img_sel"].shape[0])
         dev = self.tdevice
         z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
         lb = dict(verts=z(rows, 6890, 3), joints=z(rows, 71, 3), thetas=z(rows, 72), betas=z(rows, 11), params_pred=z(rows, N_PARAMS),
                   conf=z(rows), cam=z(rows, 3), cam_trans=z(rows, 3), pj2d_org=z(rows, 71, 2), removed=z(rows, dtype=torch.int32),
-                  sel=z(rows, dtype=torch.int32), count=z(2, dtype=torch.int32), count2=z(1, dtype=torch.int32),
-                  ctl=z(2, dtype=torch.int32), cam_full=z(self.cap, 3),
-                  ws=torch.zeros(int(self.lib.b200romp_bev_long_merge_workspace_bytes(rows)), dtype=torch.uint8, device=dev))
+                  sel=z(rows, dtype=torch.int32), count=z(2 * n_images, dtype=torch.int32), count2=z(1, dtype=torch.int32),
+                  img_sel=z(n_images, 2, dtype=torch.int32), ctl=z(2 * self.max_batch, dtype=torch.int32), cam_full=z(self.cap, 3),
+                  ws=torch.zeros(int(self.lib.b200romp_bev_long_merge_images_workspace_bytes(rows, n_images)), dtype=torch.uint8,
+                                 device=dev),
+                  host=torch.zeros(4 * n_images, dtype=torch.int32).pin_memory(), done=torch.cuda.Event())
         lb["out"] = {k: torch.zeros_like(lb[k]) for k in ("verts", "joints", "thetas", "betas", "params_pred", "conf", "cam",
                                                           "cam_trans", "pj2d_org")}
         self._long = lb
@@ -709,38 +730,69 @@ class BEV(torch.nn.Module):
 
     @torch.no_grad()
     def process_long_image(self, full_image, center3d_override=None, to_numpy=True):
-        """Crowd mode for images at least twice as wide as high, bev/main.py:184-258 (``BEV.forward`` dispatches here).
+        """Crowd mode for one image at least twice as wide as high, bev/main.py:184-258 (``BEV.forward`` dispatches
+        here): ``process_long_images([full_image])[0]``.  center3d_override: optional device [K,64,128,128] replacing
+        the crops' 3-D centre maps (tests, measurement)."""
+        return self.process_long_images([full_image], center3d_override, to_numpy)[0]
 
-        The image is zero-padded horizontally on the device and cut into the reference's overlapping crops
-        (``long_image_plan``); every crop becomes a 512x512 frame (b200romp_preprocess_bgr on the crop's window of the
-        padded image), the crops run through the model in chunks of at most ``max_batch`` frames, each chunk's
-        persons go through the per-crop filters and are appended to image-level rows (b200romp_bev_crop_post), and
-        the merged filters run on those rows (b200romp_bev_long_merge).  One host sync per image.
-        center3d_override: optional device [K,64,128,128] replacing the crops' 3-D centre maps (tests, measurement)."""
+    @torch.no_grad()
+    def process_long_images(self, images, center3d_override=None, to_numpy=True):
+        """Crowd mode for a list of images, each at least twice as wide as high (HxWx3 uint8 BGR: numpy arrays, host or
+        device tensors): element i is ``process_long_image(images[i])`` bit for bit, a dict, or None after printing
+        "No person detected!".
+
+        Every image is zero-padded horizontally on the device and cut into the reference's overlapping crops
+        (``long_images_plan``).  The list runs in passes of whole images (at most max(2 x max_batch, K of the pass's first
+        image) crops): a pass's crops, image after image, become 512x512 frames (b200romp_preprocess_bgr_batch on the
+        crops' windows of the padded images) and run through the model in chunks of at most ``max_batch`` frames that
+        may hold crops of several images; each chunk's persons go through the per-crop filters and are appended to their
+        own image's rows (b200romp_bev_crop_post_images), and the merged filters run on every image of the pass at once
+        (b200romp_bev_long_merge_images).  One host sync per pass.  center3d_override: optional device [sum K,64,128,128]
+        replacing the crops' 3-D centre maps, in crop order, image by image (tests, measurement).  ``to_numpy=False``
+        returns device tensors of the caller's current stream that own their memory (see forward_batches)."""
         if not self.calc_smpl:
             raise ValueError("the long-image mode needs SMPL (bev/main.py:203): calc_smpl must be on for images with w/h >= 2")
-        img = image_tensor(full_image)
-        s = self.settings
-        h, w = int(img.shape[0]), int(img.shape[1])
-        pad_length, boxes, pad_info = long_image_plan(h, w, s.overlap_ratio)
-        K, B = len(boxes), self.max_batch
+        imgs = [image_tensor(x) for x in images]
+        if not imgs:
+            return []
+        shapes = [(int(t.shape[0]), int(t.shape[1])) for t in imgs]
+        if any(w / h < 2 for h, w in shapes):
+            raise ValueError(f"process_long_images: every image needs w/h >= 2, got (h, w) {shapes}")
+        plan = long_images_plan(shapes, self.settings.overlap_ratio, 2 * self.max_batch)
         if center3d_override is not None:
-            assert center3d_override.is_cuda and tuple(center3d_override.shape) == (K, 64, 128, 128)
-            after_producers(self.stream, self.tdevice, center3d_override)
-        lb = self._long_buffers(K * MAX_PERSON)
-        tab = torch.from_numpy(long_image_crop_table(boxes, pad_length, h, w, float(s.nms_thresh))).pin_memory()
-        frames = frame_buffer(self.slots[self._slot]["frames"], torch.uint8, B, self.tdevice)     # free: callers drain first
+            assert center3d_override.is_cuda and tuple(center3d_override.shape) == (len(plan["boxes"]), 64, 128, 128)
+        after_producers(self.stream, self.tdevice, center3d_override, *imgs)
+        fc = plan["first_crop"]
+        self._long_buffers(max([MAX_PERSON * int(fc[i1] - fc[i0]) for i0, i1 in plan["passes"]], default=0),
+                           max([i1 - i0 for i0, i1 in plan["passes"]], default=1))
+        res = []
+        for i0, i1 in plan["passes"]:
+            res += self._long_pass(imgs, plan, i0, i1, center3d_override, to_numpy)
+        return res
+
+    def _long_pass(self, imgs, plan, i0, i1, center3d_override, to_numpy):
+        """One pass of process_long_images: images i0 .. i1-1 of the plan, their results in order."""
+        s, B, dev, lb = self.settings, self.max_batch, self.tdevice, self._long
+        fc = plan["first_crop"]
+        k0, K, n = int(fc[i0]), int(fc[i1] - fc[i0]), i1 - i0
+        boxes, pads = plan["boxes"][k0:k0 + K], plan["pad_length"]
+        tab = np.concatenate([long_image_crop_table(plan["boxes"][fc[j]:fc[j + 1]], pads[j], *imgs[j].shape[:2], float(s.nms_thresh))
+                              for j in range(i0, i1)])
+        base =(plan["row_base"][i0:i1] - plan["row_base"][i0]).astype(np.int32)
+        crops = np.stack([plan["image"][k0:k0 + K] - i0, base[plan["image"][k0:k0 + K] - i0]], 1).astype(np.int32)
+        host = [torch.from_numpy(a).pin_memory() for a in (tab, crops, plan["pad_info"][i0:i1], base)]
+        frames = frame_buffer(self.slots[self._slot]["frames"], torch.uint8, B, dev)           # free: callers drain first
         with torch.cuda.stream(self.stream):
-            padded = self.pad_long_image(img, pad_length)
-            tab_dev = tab.to(self.tdevice, non_blocking=True)
-            lb["count"].zero_()
+            padded = [self.pad_long_image(imgs[j], pads[j]) for j in range(i0, i1)]
+            tab_dev, crops_dev, pad_dev, base_dev = [t.to(dev, non_blocking=True) for t in host]
+            lb["count"][:2 * n].zero_()
             for c0 in range(0, K, B):
                 nb = min(B, K - c0)
-                self.crop_frames(padded, boxes[c0:c0 + nb], frames)                         # main.py:197-199 + img_preprocess
-                self.run_model(frames[:nb], None if center3d_override is None else center3d_override[c0:c0 + nb])
-                self.crop_post(nb, c0, tab_dev)
-            self.long_merge(pad_info, w)
-        return self._collect_long(to_numpy)
+                self.crop_frames([padded[i] for i in crops[c0:c0 + nb, 0]], boxes[c0:c0 + nb], frames)   # main.py:197-199
+                self.run_model(frames[:nb], None if center3d_override is None else center3d_override[k0 + c0:k0 + c0 + nb])
+                self.crop_post(nb, c0, tab_dev, crops_dev)
+            self.long_merge_images(pad_dev, base_dev, MAX_PERSON * int(np.max(np.diff(fc[i0:i1 + 1]))))
+        return self._collect_long_images(n, to_numpy)
 
     def pad_long_image(self, img, pad_length):
         """padding_image_overlap (split2process.py:6-13) on the device: h x (w + 2*pad_length) x 3, zero columns each side."""
@@ -752,51 +804,93 @@ class BEV(torch.nn.Module):
 
     def crop_frames(self, padded, boxes, frames):
         """frames[i] = img_preprocess(padded[t:b, l:r]) for box i: one b200romp_preprocess_bgr_batch call for all the boxes,
-        each crop a window of the padded image (its own size, the padded row stride)."""
-        crops = [padded[t:b, l:r] for l, r, t, b in np.asarray(boxes).tolist()]
+        each crop a window of the padded image (its own size, the padded row stride).  ``padded``: one padded image, or
+        a list with the padded image of every box."""
+        padded = padded if isinstance(padded, list) else [padded] * len(boxes)
+        crops = [p[t:b, l:r] for p, (l, r, t, b) in zip(padded, np.asarray(boxes).tolist())]
         preprocess_bgr_batch(self.lib, crops, [None] * len(crops), None, frames, None, self.stream.cuda_stream)
 
-    def crop_post(self, nb, crop0, tab_dev):
-        """SMPL-A / SMIL on the chunk's persons, then the per-crop stage (b200romp_bev_crop_post): survivors appended to
-        the image-level rows."""
+    def crop_post(self, nb, crop0, tab_dev, crops_dev=None):
+        """SMPL-A / SMIL on the chunk's persons, then the per-crop stage: survivors appended to the image-level rows.
+        ``crops_dev``: the pass's device int32 [K,2] {image, first row} table (b200romp_bev_crop_post_images); None for
+        the crops of one image (b200romp_bev_crop_post)."""
         lib, b, lb, st = self.lib, self.buf, self._long, self.stream.cuda_stream
         cap = nb * MAX_PERSON
         self.smpla.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts"], b["joints"], st)
         self.smil.forward(b["betas"], b["thetas"], cap, b["count"], True, b["smpl_ws"], b["verts_smil"], b["joints_smil"], st)
-        _lib.check(lib.b200romp_bev_crop_post(
-            _ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]), _ptr(b["joints"]),
-            _ptr(b["thetas"]), _ptr(b["params_pred"]), _ptr(b["conf"]), _ptr(b["cam"]), _ptr(b["cam_trans"]),
-            _ptr(b["batch_ids"]), nb, cap, _ptr(b["count"]), _ptr(tab_dev), crop0, float(self.settings.relative_scale_thresh),
-            _ptr(b["pj2d_org"]), _ptr(b["keep"]), _ptr(b["sel"]), _ptr(lb["cam_full"]), lb["cam"].shape[0], _ptr(lb["count"]),
-            _ptr(lb["ctl"]), _ptr(lb["verts"]), _ptr(lb["joints"]), _ptr(lb["thetas"]), _ptr(lb["betas"]),
-            _ptr(lb["params_pred"]), _ptr(lb["conf"]), _ptr(lb["cam"]), C.c_void_p(st)), "bev_crop_post")
+        rows = (_ptr(b["betas"]), _ptr(b["verts_smil"]), _ptr(b["joints_smil"]), _ptr(b["verts"]), _ptr(b["joints"]),
+                _ptr(b["thetas"]), _ptr(b["params_pred"]), _ptr(b["conf"]), _ptr(b["cam"]), _ptr(b["cam_trans"]),
+                _ptr(b["batch_ids"]), nb, cap, _ptr(b["count"]), _ptr(tab_dev))
+        acc = (crop0, float(self.settings.relative_scale_thresh), _ptr(b["pj2d_org"]), _ptr(b["keep"]), _ptr(b["sel"]),
+               _ptr(lb["cam_full"]), lb["cam"].shape[0], _ptr(lb["count"]), _ptr(lb["ctl"]), _ptr(lb["verts"]), _ptr(lb["joints"]),
+               _ptr(lb["thetas"]), _ptr(lb["betas"]), _ptr(lb["params_pred"]), _ptr(lb["conf"]), _ptr(lb["cam"]), C.c_void_p(st))
+        if crops_dev is None:
+            _lib.check(lib.b200romp_bev_crop_post(*rows, *acc), "bev_crop_post")
+        else:
+            _lib.check(lib.b200romp_bev_crop_post_images(*rows, _ptr(crops_dev), *acc), "bev_crop_post_images")
 
     @torch.no_grad()
     def long_merge(self, pad_info, img_max_side):
-        """Merged stage of the long-image mode (bev/main.py:253-256) on the accumulated rows, then row compaction."""
-        lib, lb, sp = self.lib, self._long, C.c_void_p(self.stream.cuda_stream)
-        rows = lb["cam"].shape[0]
+        """Merged stage of the long-image mode (bev/main.py:253-256) on one image's accumulated rows, then row
+        compaction: the one-image case of ``long_merge_images`` (b200romp_bev_long_merge, the count kept to img_sel[0])."""
+        lb = self._long
         off = (C.c_float * 6)(*[float(v) for v in pad_info])
-        _lib.check(lib.b200romp_bev_long_merge(_ptr(lb["cam"]), _ptr(lb["joints"]), _ptr(lb["conf"]), rows, _ptr(lb["count"]), off,
-                                               float(self.settings.nms_thresh), float(self.settings.relative_scale_thresh),
-                                               float(img_max_side), _ptr(lb["cam_trans"]), _ptr(lb["pj2d_org"]), _ptr(lb["removed"]),
-                                               _ptr(lb["ws"]), _ptr(lb["sel"]), _ptr(lb["count2"]), sp), "bev_long_merge")
+        _lib.check(self.lib.b200romp_bev_long_merge(
+            _ptr(lb["cam"]), _ptr(lb["joints"]), _ptr(lb["conf"]), lb["cam"].shape[0], _ptr(lb["count"]), off,
+            float(self.settings.nms_thresh), float(self.settings.relative_scale_thresh), float(img_max_side), _ptr(lb["cam_trans"]),
+            _ptr(lb["pj2d_org"]), _ptr(lb["removed"]), _ptr(lb["ws"]), _ptr(lb["sel"]), _ptr(lb["img_sel"][0, 1:]),
+            C.c_void_p(self.stream.cuda_stream)), "bev_long_merge")
+        self._gather_long(lb["img_sel"][0, 1:])
+
+    @torch.no_grad()
+    def long_merge_images(self, pad_dev, base_dev, image_rows):
+        """Merged stage of a pass (b200romp_bev_long_merge_images) on the accumulated rows of its images (device pad
+        table [n,6], device int32 first rows [n], at most image_rows rows per image), then one row compaction for all."""
+        lb = self._long
+        _lib.check(self.lib.b200romp_bev_long_merge_images(
+            _ptr(lb["cam"]), _ptr(lb["joints"]), _ptr(lb["conf"]), lb["cam"].shape[0], len(base_dev), image_rows, _ptr(base_dev),
+            _ptr(lb["count"]), _ptr(pad_dev), float(self.settings.nms_thresh), float(self.settings.relative_scale_thresh),
+            _ptr(lb["cam_trans"]), _ptr(lb["pj2d_org"]), _ptr(lb["removed"]), _ptr(lb["ws"]), _ptr(lb["sel"]), _ptr(lb["img_sel"]),
+            _ptr(lb["count2"]), C.c_void_p(self.stream.cuda_stream)), "bev_long_merge_images")
+        self._gather_long(lb["count2"])
+
+    def _gather_long(self, count):
+        """lb["out"][k][i] = lb[k][sel[i]] for i < count (device int32 [1]), one launch per field."""
+        lb, sp = self._long, C.c_void_p(self.stream.cuda_stream)
         for k, dst in lb["out"].items():
             src = lb[k]
             row = src[0].numel() * src.element_size()
-            _lib.check(lib.b200romp_gather_rows(_ptr(src), row, _ptr(lb["sel"]), _ptr(lb["count2"]), rows, _ptr(dst), sp), "gather_rows")
+            _lib.check(self.lib.b200romp_gather_rows(_ptr(src), row, _ptr(lb["sel"]), _ptr(count), src.shape[0], _ptr(dst), sp),
+                       "gather_rows")
 
     def _collect_long(self, to_numpy=True):
-        lb = self._long
-        n_det, n = self._counts(lb["count"][1:2], lb["count2"])      # persons detected in any crop, persons kept
-        if n_det == 0:                        # the reference raises KeyError here (main.py:253); INTEGRATION.md, Deviations
-            print("No person detected!")
-            return None
-        out = self._result(lb["out"], n, torch.zeros(n, dtype=torch.int64, device=self.tdevice))
+        """The result of one image's merged stage (``long_merge``)."""
+        return self._collect_long_images(1, to_numpy)[0]
+
+    def _collect_long_images(self, n, to_numpy=True):
+        """The results of a pass's n images from its merged stage: one host sync for the persons detected in each image's
+        crops and the start and count of its kept rows, then each image's rows (arrays, or copies on the caller's stream)."""
+        lb, h = self._long, self._long["host"]
+        with torch.cuda.stream(self.stream):
+            h[:2 * n].copy_(lb["count"][:2 * n], non_blocking=True)
+            h[2 * n:4 * n].copy_(lb["img_sel"][:n].reshape(-1), non_blocking=True)
+            lb["done"].record(self.stream)
+        self.stream.synchronize()
+        det, start, kept = h[1:2 * n:2].tolist(), h[2 * n:4 * n:2].tolist(), h[2 * n + 1:4 * n:2].tolist()
+        src = lb["out"]
         if to_numpy:
             with torch.cuda.stream(self.stream):
-                out = {k: v.contiguous().cpu().numpy() for k, v in out.items()}
-        return out
+                src = {k: v[:start[-1] + kept[-1]].cpu().numpy() for k, v in src.items()}
+        res = []
+        for j in range(n):
+            if det[j] == 0:                   # the reference raises KeyError here (main.py:253); INTEGRATION.md, Deviations
+                print("No person detected!")
+                res.append(None)
+                continue
+            s, k = start[j], kept[j]
+            ids = np.zeros(k, np.int64) if to_numpy else torch.zeros(k, dtype=torch.int64, device=self.tdevice)
+            res.append(self._result({key: v[s:] for key, v in src.items()}, k, ids))
+        return res if to_numpy else to_caller(res, lb["done"], self.stream)
 
     @torch.no_grad()
     def forward(self, image, signal_ID=0, **kwargs):

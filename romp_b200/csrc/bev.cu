@@ -667,36 +667,95 @@ __device__ int block_compact(int n, Flag flag, Val val, int* __restrict__ out) {
   return s_base;
 }
 
-// append the chunk's survivors at the image's running count acc_count[0]: sel = their chunk rows, ctl = {base, n_new}
+// The crops of several images in one pass: crop_img [n_crops][2] int32 = {image, first accumulation row of that image}
+// per crop, images in crop order.  NULL: every crop belongs to image 0, whose rows start at 0.
+__device__ __forceinline__ int crop_image(const int* __restrict__ crop_img, int c) { return crop_img ? crop_img[2 * c] : 0; }
+
+// Append the chunk's survivors image by image (the chunk's l-th image is image j0 + l) at each image's running count
+// acc_count[2j] (rows from its first row, all images together at most acc_capacity rows); acc_count[2j+1] counts the
+// image's persons detected so far, survivors or not.  sel = the chunk rows of all survivors in order; survivor i of the
+// l-th image goes to row ctl[2l] + i if i < ctl[2l+1] (one image: ctl = {first row, rows appended}).
 __global__ void __launch_bounds__(1024) bev_crop_append_kernel(const int* __restrict__ keep, const int* __restrict__ d_count,
-                                                               int acc_capacity, int* __restrict__ acc_count, int* __restrict__ sel,
-                                                               int* __restrict__ ctl) {
-  const int N = *d_count;
-  const int k = block_compact(N, [&](int i) { return keep[i] != 0; }, [](int i) { return i; }, sel);
-  if (threadIdx.x == 0) {
-    const int base = *acc_count, n = min(k, acc_capacity - base);
-    ctl[0] = base; ctl[1] = n;
-    acc_count[0] = base + n;
-    acc_count[1] += N;                    // persons detected in the image so far, survivors or not
+                                                               const long long* __restrict__ batch_ids, const int* __restrict__ crop_img,
+                                                               int crop0, int batch, int acc_capacity, int* __restrict__ acc_count,
+                                                               int* __restrict__ sel, int* __restrict__ ctl) {
+  __shared__ int s_b0, s_b1, s_r0, s_r1, s_k;
+  const int N = *d_count, j0 = crop_image(crop_img, crop0), nl = crop_image(crop_img, crop0 + batch - 1) - j0 + 1;
+  if (threadIdx.x == 0) { s_b1 = 0; s_r1 = 0; s_k = 0; }
+  for (int l = 0; l < nl; ++l) {
+    if (threadIdx.x == 0) {            // the l-th image's crops [s_b0, s_b1) of the chunk and rows [s_r0, s_r1)
+      int b = s_b1, lo = s_r1, hi = N;
+      s_b0 = b; s_r0 = lo;
+      while (b < batch && crop_image(crop_img, crop0 + b) == j0 + l) ++b;
+      s_b1 = b;
+      while (l < nl - 1 && lo < hi) {  // rows are grouped by frame in frame order; the last image's end at N
+        const int mid = (lo + hi) >> 1;
+        if (batch_ids[mid] < b) lo = mid + 1; else hi = mid;
+      }
+      s_r1 = l < nl - 1 ? lo : N;
+    }
+    __syncthreads();
+    const int r0 = s_r0, r1 = s_r1, k0 = s_k;
+    const int k = block_compact(r1 - r0, [&](int i) { return keep[r0 + i] != 0; }, [&](int i) { return r0 + i; }, sel + k0);
+    if (threadIdx.x == 0) {
+      const int j = j0 + l, first = crop_img ? crop_img[2 * (crop0 + s_b0) + 1] : 0;
+      const int have = acc_count[2 * j], n = min(k, acc_capacity - first - have);
+      ctl[2 * l] = first + have - k0; ctl[2 * l + 1] = k0 + n;
+      acc_count[2 * j] = have + n;
+      acc_count[2 * j + 1] += r1 - r0;
+      s_k = k0 + k;
+    }
   }
 }
 
 __global__ void __launch_bounds__(256) append_rows_kernel(const uint32_t* __restrict__ src, int row_words, const int* __restrict__ sel,
-                                                          const int* __restrict__ ctl, uint32_t* __restrict__ dst) {
-  const int i = blockIdx.x;
-  if (i >= ctl[1]) return;
+                                                          const int* __restrict__ ctl, const long long* __restrict__ batch_ids,
+                                                          const int* __restrict__ crop_img, int crop0, int batch,
+                                                          uint32_t* __restrict__ dst) {
+  const int i = blockIdx.x, j0 = crop_image(crop_img, crop0);
+  // the appended survivors of the chunk's images end at nondecreasing ctl[2l+1], so past the last image's end is past all
+  if (i >= ctl[2 * (crop_image(crop_img, crop0 + batch - 1) - j0) + 1]) return;
+  const int l = crop_img ? crop_image(crop_img, crop0 + (int)batch_ids[sel[i]]) - j0 : 0;
+  if (i >= ctl[2 * l + 1]) return;
   const uint32_t* s = src + (size_t)sel[i] * row_words;
-  uint32_t* d = dst + (size_t)(ctl[0] + i) * row_words;
+  uint32_t* d = dst + (size_t)(ctl[2 * l] + i) * row_words;
   for (int k = blockIdx.y * 256 + threadIdx.x; k < row_words; k += gridDim.y * 256) d[k] = s[k];
 }
 
+// The merged stage runs over the accumulated rows of n_images images at once: image j's rows start at row_base[j]
+// (row_base NULL: one image, rows from 0) and it has d_count[2j] of them (the crop stage's acc_count).  With pad_tab
+// (device [n_images,6]) image j projects with its own pad info and suppresses with its own max(h, w), else every row
+// uses the shared size / left / top / nms_thr_px.
+struct LongImages {
+  int n;
+  const int* row_base;
+  const int* count;
+  const float* pad_tab;
+  double nms_thresh;
+  __device__ int first_row(int img) const { return row_base ? row_base[img] : 0; }
+  __device__ int rows(int img) const { return count[2 * img]; }
+  __device__ int of_row(int r) const {          // the image of accumulation row r
+    int lo = 0, hi = row_base ? n - 1 : 0;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (row_base[mid] <= r) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+  }
+};
+
 // merged stage, bev/main.py:253-256: cam_trans from the full-image cam and projection with the full image's pad info
 __global__ void __launch_bounds__(128) bev_long_project_kernel(const float* __restrict__ cam, const float* __restrict__ joints,
-                                                               const int* __restrict__ d_count, float size, float left, float top,
+                                                               LongImages im, float size, float left, float top,
                                                                float* __restrict__ cam_trans, float* __restrict__ pj2d_org,
                                                                int* __restrict__ removed) {
-  const int n = blockIdx.x, j = threadIdx.x;
-  if (n >= *d_count) return;
+  const int n = blockIdx.x, j = threadIdx.x, img = im.of_row(n);
+  if (n - im.first_row(img) >= im.rows(img)) return;
+  if (im.pad_tab) {
+    const float* f = im.pad_tab + img * 6;
+    top = f[0]; left = f[2];
+    size = f[4] > f[5] ? f[4] : f[5];
+  }
   float tr[3];
   bev_cam_trans_rn(cam + n * 3, tr);                    // denormalize_cam_params_to_trans (bev/post_parser.py:114-128)
   const float tx = tr[0], ty = tr[1], depth = tr[2];
@@ -712,16 +771,19 @@ __global__ void __launch_bounds__(128) bev_long_project_kernel(const float* __re
   pj2d_org[((size_t)n * 71 + j) * 2 + 1] = (v + 1.f) * size / 2.f - top;
 }
 
-// conf-based suppression over ALL accumulated persons (not bounded by 64): one 16 x 16 tile of pairs (i < j) per CTA; every
-// pair below the threshold removes its lower-confidence member, all pairs at once like the reference's torch.where
+// conf-based suppression over ALL accumulated persons of an image (not bounded by 64): one 16 x 16 tile of pairs (i < j)
+// per CTA, images on blockIdx.z; every pair below the threshold removes its lower-confidence member, all pairs at once like
+// the reference's torch.where
 constexpr int kPT = 16;
 __global__ void __launch_bounds__(256) bev_long_pairs_kernel(const float* __restrict__ pj2d_org, const float* __restrict__ cam,
-                                                             const float* __restrict__ conf, const int* __restrict__ d_count,
-                                                             float nms_thr_px, int* __restrict__ removed) {
+                                                             const float* __restrict__ conf, LongImages im, float nms_thr_px,
+                                                             int* __restrict__ removed) {
   __shared__ float s_a[kPT][142], s_b[kPT][142];
-  const int N = *d_count;
+  const int img = blockIdx.z, N = im.rows(img), first = im.first_row(img);
   const int i0 = blockIdx.y * kPT, j0 = blockIdx.x * kPT;
   if (i0 >= N || j0 >= N || j0 + kPT - 1 <= i0) return;
+  if (im.pad_tab) nms_thr_px = nms_thr_px_of(im.nms_thresh, fmaxf(im.pad_tab[img * 6 + 4], im.pad_tab[img * 6 + 5]));
+  pj2d_org += (size_t)first * 142; cam += (size_t)first * 3; conf += first; removed += first;
   for (int t = threadIdx.x; t < kPT * 142; t += 256) {
     const int r = t / 142, c = t % 142;
     s_a[r][c] = i0 + r < N ? pj2d_org[(size_t)(i0 + r) * 142 + c] : 0.f;
@@ -739,21 +801,24 @@ __global__ void __launch_bounds__(256) bev_long_pairs_kernel(const float* __rest
   if (sum / 71.f / fmaxf(si, sj) < nms_thr_px) removed[conf[i] < conf[j] ? i : j] = 1;
 }
 
-// survivors of the suppression: ws_sel[0, nk), *ws_nk = nk
-__global__ void __launch_bounds__(1024) bev_long_kept_kernel(const int* __restrict__ removed, const int* __restrict__ d_count,
-                                                             int* __restrict__ ws_sel, int* __restrict__ ws_nk) {
-  const int k = block_compact(*d_count, [&](int i) { return removed[i] == 0; }, [](int i) { return i; }, ws_sel);
-  if (threadIdx.x == 0) *ws_nk = k;
+// survivors of the suppression, one CTA per image: the image's rows ws_sel[first, first + nk), ws_nk[img] = nk
+__global__ void __launch_bounds__(1024) bev_long_kept_kernel(const int* __restrict__ removed, LongImages im, int* __restrict__ ws_sel,
+                                                             int* __restrict__ ws_nk) {
+  const int img = blockIdx.x, first = im.first_row(img);
+  const int k = block_compact(im.rows(img), [&](int i) { return removed[first + i] == 0; }, [&](int i) { return first + i; },
+                              ws_sel + first);
+  if (threadIdx.x == 0) ws_nk[img] = k;
 }
 
-// remove_outlier, mean of each survivor's sorted distance row without its first and last entry: one CTA per survivor.
-// The first entry is the self-distance (exactly 0), the last the row maximum; the row is summed without the first index
-// that attains the maximum (a (max, smallest index) reduction, then a second pass), so a far person does not cancel
-// against the sum the way (sum - min - max) does.
+// remove_outlier, mean of each survivor's sorted distance row without its first and last entry: one CTA per survivor,
+// images on blockIdx.y.  The first entry is the self-distance (exactly 0), the last the row maximum; the row is summed
+// without the first index that attains the maximum (a (max, smallest index) reduction, then a second pass), so a far
+// person does not cancel against the sum the way (sum - min - max) does.
 __global__ void __launch_bounds__(128) bev_long_meandist_kernel(const float* __restrict__ cam_trans, const int* __restrict__ ws_sel,
-                                                                const int* __restrict__ ws_nk, float* __restrict__ ws_mean) {
-  const int nk = *ws_nk, r = blockIdx.x;
+                                                                const int* __restrict__ ws_nk, float* __restrict__ ws_mean, LongImages im) {
+  const int img = blockIdx.y, nk = ws_nk[img], r = blockIdx.x, first = im.first_row(img);
   if (nk < 3 || r >= nk) return;
+  ws_sel += first; ws_mean += first;
   const float* ti = cam_trans + (size_t)ws_sel[r] * 3;
   auto dist = [&](int k) {
     const float* tj = cam_trans + (size_t)ws_sel[k] * 3;
@@ -790,14 +855,16 @@ __global__ void __launch_bounds__(128) bev_long_meandist_kernel(const float* __r
   if (threadIdx.x == 0) ws_mean[r] = (s_sum[0] + s_sum[1] + s_sum[2] + s_sum[3]) / (float)(nk - 2);
 }
 
-// relative scale of every survivor against the others, outliers (and cam[:,0] < scale_thresh) removed, final compaction
+// relative scale of every survivor against the others, outliers (and cam[:,0] < scale_thresh) removed, final compaction:
+// one CTA per image, its kept rows at sel[first, first + n), n_out[2 img] = n
 __global__ void __launch_bounds__(1024) bev_long_outlier_kernel(const float* __restrict__ cam, const int* __restrict__ ws_sel,
                                                                 const int* __restrict__ ws_nk, const float* __restrict__ ws_mean,
-                                                                float rel_scale_thresh, float scale_thresh, int* __restrict__ sel,
-                                                                int* __restrict__ d_count_out) {
+                                                                float rel_scale_thresh, float scale_thresh, LongImages im,
+                                                                int* __restrict__ sel, int* __restrict__ n_out) {
   __shared__ float s_part[32];
   __shared__ float s_tot;
-  const int nk = *ws_nk, tid = threadIdx.x;
+  const int img = blockIdx.x, nk = ws_nk[img], tid = threadIdx.x, first = im.first_row(img);
+  ws_sel += first; ws_mean += first; sel += first;
   float tot = 0.f;
   if (nk >= 3) {
     for (int k = tid; k < nk; k += blockDim.x) tot += ws_mean[k];
@@ -819,7 +886,27 @@ __global__ void __launch_bounds__(1024) bev_long_outlier_kernel(const float* __r
     return !(rel > rel_scale_thresh && cam[ws_sel[k] * 3] < scale_thresh);
   };
   const int n = block_compact(nk, keep, [&](int k) { return ws_sel[k]; }, sel);
-  if (tid == 0) *d_count_out = n;
+  if (tid == 0) n_out[2 * img] = n;
+}
+
+// the images' kept rows, each at sel[first row of the image, + count), moved to one run in image order:
+// img_sel[img] = {start, count}, *d_count_out = the total.  Rows only move down, a block at a time, so in place is safe.
+__global__ void __launch_bounds__(1024) bev_long_pack_kernel(LongImages im, int* __restrict__ sel, int* __restrict__ img_sel,
+                                                             int* __restrict__ d_count_out) {
+  int start = 0;
+  for (int img = 0; img < im.n; ++img) {
+    const int first = im.first_row(img), n = img_sel[2 * img + 1];
+    for (int c = 0; c < n; c += blockDim.x) {
+      const int t = c + threadIdx.x;
+      const int v = t < n ? sel[first + t] : 0;
+      __syncthreads();
+      if (t < n) sel[start + t] = v;
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) img_sel[2 * img] = start;
+    start += n;
+  }
+  if (threadIdx.x == 0) *d_count_out = start;
 }
 
 __global__ void bev_compact_kernel(const int* __restrict__ keep, const int* __restrict__ d_count, int* __restrict__ sel,
@@ -1018,6 +1105,30 @@ int b200romp_bev_post_frames(const float* betas, const float* verts_smil, const 
                   nms_thresh, rel_scale_thresh, 0.f, pj2d_org, keep, sel, d_count_out, (cudaStream_t)stream_);
 }
 
+// the per-crop stage of one chunk; crop_img NULL: the crops of one image (b200romp_bev_crop_post)
+static int bev_crop_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                         const float* thetas, const float* params_pred, const float* conf, const float* cam, const float* cam_trans,
+                         const long long* batch_ids, int batch, int capacity, const int* d_count, const float* crop_table,
+                         const int* crop_img, int crop0, float rel_scale_thresh, float* pj2d, int* keep, int* sel, float* cam_full,
+                         int acc_capacity, int* acc_count, int* acc_ctl, float* acc_verts, float* acc_joints, float* acc_thetas,
+                         float* acc_betas, float* acc_params_pred, float* acc_conf, float* acc_cam, cudaStream_t stream) {
+  if (verts_smil && joints_smil)
+    bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
+  B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
+  bev_crop_filter_kernel<<<batch, 256, 0, stream>>>(joints, cam, cam_trans, conf, batch_ids, d_count, crop_table, crop0,
+                                                    rel_scale_thresh, pj2d, keep, cam_full);
+  bev_crop_append_kernel<<<1, 1024, 0, stream>>>(keep, d_count, batch_ids, crop_img, crop0, batch, acc_capacity, acc_count, sel, acc_ctl);
+  const struct { const void* src; void* dst; int words; } rows[] = {
+      {verts, acc_verts, 6890 * 3}, {joints, acc_joints, 71 * 3}, {thetas, acc_thetas, 72}, {betas, acc_betas, 11},
+      {params_pred, acc_params_pred, 146}, {conf, acc_conf, 1}, {cam_full, acc_cam, 3}};
+  for (const auto& r : rows)
+    append_rows_kernel<<<dim3(capacity, r.words > 4096 ? 8 : 1), 256, 0, stream>>>(
+        reinterpret_cast<const uint32_t*>(r.src), r.words, sel, acc_ctl, batch_ids, crop_img, crop0, batch,
+        reinterpret_cast<uint32_t*>(r.dst));
+  B2R_CUDA_OK(cudaGetLastError());
+  return B200ROMP_OK;
+}
+
 int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
                            const float* thetas, const float* params_pred, const float* conf, const float* cam, const float* cam_trans,
                            const long long* batch_ids, int batch, int capacity, const int* d_count, const float* crop_table,
@@ -1028,44 +1139,82 @@ int b200romp_bev_crop_post(const float* betas, const float* verts_smil, const fl
                   pj2d && keep && sel && cam_full && acc_count && acc_ctl && acc_verts && acc_joints && acc_thetas && acc_betas &&
                   acc_params_pred && acc_conf && acc_cam && batch > 0 && capacity > 0 && crop0 >= 0 && acc_capacity > 0,
               "bev_crop_post: bad arguments");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (verts_smil && joints_smil)
-    bev_merge_smil_kernel<<<dim3(capacity, 4), 256, 0, stream>>>(betas, d_count, verts_smil, joints_smil, verts, joints);
-  B2R_CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int) * capacity, stream));
-  bev_crop_filter_kernel<<<batch, 256, 0, stream>>>(joints, cam, cam_trans, conf, batch_ids, d_count, crop_table, crop0,
-                                                    rel_scale_thresh, pj2d, keep, cam_full);
-  bev_crop_append_kernel<<<1, 1024, 0, stream>>>(keep, d_count, acc_capacity, acc_count, sel, acc_ctl);
-  const struct { const void* src; void* dst; int words; } rows[] = {
-      {verts, acc_verts, 6890 * 3}, {joints, acc_joints, 71 * 3}, {thetas, acc_thetas, 72}, {betas, acc_betas, 11},
-      {params_pred, acc_params_pred, 146}, {conf, acc_conf, 1}, {cam_full, acc_cam, 3}};
-  for (const auto& r : rows)
-    append_rows_kernel<<<dim3(capacity, r.words > 4096 ? 8 : 1), 256, 0, stream>>>(
-        reinterpret_cast<const uint32_t*>(r.src), r.words, sel, acc_ctl, reinterpret_cast<uint32_t*>(r.dst));
+  return bev_crop_post(betas, verts_smil, joints_smil, verts, joints, thetas, params_pred, conf, cam, cam_trans, batch_ids, batch,
+                       capacity, d_count, crop_table, nullptr, crop0, rel_scale_thresh, pj2d, keep, sel, cam_full, acc_capacity,
+                       acc_count, acc_ctl, acc_verts, acc_joints, acc_thetas, acc_betas, acc_params_pred, acc_conf, acc_cam,
+                       (cudaStream_t)stream_);
+}
+
+int b200romp_bev_crop_post_images(const float* betas, const float* verts_smil, const float* joints_smil, float* verts, float* joints,
+                                  const float* thetas, const float* params_pred, const float* conf, const float* cam,
+                                  const float* cam_trans, const long long* batch_ids, int batch, int capacity, const int* d_count,
+                                  const float* crop_table, const int* crop_images, int crop0, float rel_scale_thresh, float* pj2d,
+                                  int* keep, int* sel, float* cam_full, int acc_capacity, int* acc_count, int* acc_ctl,
+                                  float* acc_verts, float* acc_joints, float* acc_thetas, float* acc_betas, float* acc_params_pred,
+                                  float* acc_conf, float* acc_cam, b200romp_stream stream_) {
+  B2R_REQUIRE(betas && verts && joints && thetas && params_pred && conf && cam && cam_trans && batch_ids && d_count && crop_table &&
+                  crop_images && pj2d && keep && sel && cam_full && acc_count && acc_ctl && acc_verts && acc_joints && acc_thetas &&
+                  acc_betas && acc_params_pred && acc_conf && acc_cam && batch > 0 && capacity > 0 && crop0 >= 0 && acc_capacity > 0,
+              "bev_crop_post_images: bad arguments");
+  return bev_crop_post(betas, verts_smil, joints_smil, verts, joints, thetas, params_pred, conf, cam, cam_trans, batch_ids, batch,
+                       capacity, d_count, crop_table, crop_images, crop0, rel_scale_thresh, pj2d, keep, sel, cam_full, acc_capacity,
+                       acc_count, acc_ctl, acc_verts, acc_joints, acc_thetas, acc_betas, acc_params_pred, acc_conf, acc_cam,
+                       (cudaStream_t)stream_);
+}
+
+// workspace: ws_nk [n_images] (padded to 4 ints), then ws_sel [capacity], ws_mean [capacity]
+long long b200romp_bev_long_merge_images_workspace_bytes(int capacity, int n_images) {
+  return (long long)capacity * 8 + 16LL * ((n_images + 3) / 4);
+}
+
+long long b200romp_bev_long_merge_workspace_bytes(int capacity) { return b200romp_bev_long_merge_images_workspace_bytes(capacity, 1); }
+
+// the merged stage of one pass; one image (b200romp_bev_long_merge): row_base and pad_table NULL, the host pad info and
+// img_max_side, no img_sel (the kept count goes to *d_count_out)
+static int bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, int image_rows, LongImages im,
+                          const float* offsets6, float img_max_side, float rel_scale_thresh, float* cam_trans, float* pj2d_org,
+                          int* removed, void* workspace, int* sel, int* img_sel, int* d_count_out, cudaStream_t stream) {
+  int* ws_nk = reinterpret_cast<int*>(workspace);
+  int* ws_sel = ws_nk + 4 * ((im.n + 3) / 4);
+  float* ws_mean = reinterpret_cast<float*>(ws_sel + capacity);
+  float top = 0.f, left = 0.f, size = 0.f;
+  if (offsets6) {
+    const float hh = offsets6[4], ww = offsets6[5];
+    top = offsets6[0]; left = offsets6[2]; size = hh > ww ? hh : ww;
+  }
+  bev_long_project_kernel<<<capacity, 128, 0, stream>>>(cam, joints, im, size, left, top, cam_trans, pj2d_org, removed);
+  const unsigned tiles = (unsigned)((image_rows + kPT - 1) / kPT);
+  const float thr_px = offsets6 ? nms_thr_px_of(im.nms_thresh, img_max_side) : 0.f;      // a pad table gives each image its own
+  bev_long_pairs_kernel<<<dim3(tiles, tiles, im.n), 256, 0, stream>>>(pj2d_org, cam, conf, im, thr_px, removed);
+  bev_long_kept_kernel<<<im.n, 1024, 0, stream>>>(removed, im, ws_sel, ws_nk);
+  bev_long_meandist_kernel<<<dim3(image_rows, im.n), 128, 0, stream>>>(cam_trans, ws_sel, ws_nk, ws_mean, im);
+  bev_long_outlier_kernel<<<im.n, 1024, 0, stream>>>(cam, ws_sel, ws_nk, ws_mean, rel_scale_thresh, 0.5f, im, sel,
+                                                     img_sel ? img_sel + 1 : d_count_out);
+  if (img_sel) bev_long_pack_kernel<<<1, 1024, 0, stream>>>(im, sel, img_sel, d_count_out);
   B2R_CUDA_OK(cudaGetLastError());
   return B200ROMP_OK;
 }
-
-long long b200romp_bev_long_merge_workspace_bytes(int capacity) { return (long long)capacity * 8 + 16; }
 
 int b200romp_bev_long_merge(const float* cam, const float* joints, const float* conf, int capacity, const int* d_count,
                             const float* offsets6, double nms_thresh, float rel_scale_thresh, float img_max_side, float* cam_trans,
                             float* pj2d_org, int* removed, void* workspace, int* sel, int* d_count_out, b200romp_stream stream_) {
   B2R_REQUIRE(cam && joints && conf && d_count && offsets6 && cam_trans && pj2d_org && removed && workspace && sel && d_count_out &&
                   capacity > 0 && img_max_side > 0.f, "bev_long_merge: bad arguments");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  int* ws_nk = reinterpret_cast<int*>(workspace);
-  int* ws_sel = ws_nk + 4;
-  float* ws_mean = reinterpret_cast<float*>(ws_sel + capacity);
-  const float top = offsets6[0], left = offsets6[2], hh = offsets6[4], ww = offsets6[5];
-  bev_long_project_kernel<<<capacity, 128, 0, stream>>>(cam, joints, d_count, hh > ww ? hh : ww, left, top, cam_trans, pj2d_org, removed);
-  const unsigned tiles = (unsigned)((capacity + kPT - 1) / kPT);
-  bev_long_pairs_kernel<<<dim3(tiles, tiles), 256, 0, stream>>>(pj2d_org, cam, conf, d_count, nms_thr_px_of(nms_thresh, img_max_side),
-                                                                removed);
-  bev_long_kept_kernel<<<1, 1024, 0, stream>>>(removed, d_count, ws_sel, ws_nk);
-  bev_long_meandist_kernel<<<capacity, 128, 0, stream>>>(cam_trans, ws_sel, ws_nk, ws_mean);
-  bev_long_outlier_kernel<<<1, 1024, 0, stream>>>(cam, ws_sel, ws_nk, ws_mean, rel_scale_thresh, 0.5f, sel, d_count_out);
-  B2R_CUDA_OK(cudaGetLastError());
-  return B200ROMP_OK;
+  return bev_long_merge(cam, joints, conf, capacity, capacity, LongImages{1, nullptr, d_count, nullptr, nms_thresh}, offsets6,
+                        img_max_side, rel_scale_thresh, cam_trans, pj2d_org, removed, workspace, sel, nullptr, d_count_out,
+                        (cudaStream_t)stream_);
+}
+
+int b200romp_bev_long_merge_images(const float* cam, const float* joints, const float* conf, int capacity, int n_images,
+                                   int image_rows, const int* row_base, const int* acc_count, const float* pad_table, double nms_thresh,
+                                   float rel_scale_thresh, float* cam_trans, float* pj2d_org, int* removed, void* workspace, int* sel,
+                                   int* img_sel, int* d_count_out, b200romp_stream stream_) {
+  B2R_REQUIRE(cam && joints && conf && row_base && acc_count && pad_table && cam_trans && pj2d_org && removed && workspace && sel &&
+                  img_sel && d_count_out && capacity > 0 && n_images > 0 && image_rows > 0 && image_rows <= capacity,
+              "bev_long_merge_images: bad arguments");
+  return bev_long_merge(cam, joints, conf, capacity, image_rows, LongImages{n_images, row_base, acc_count, pad_table, nms_thresh},
+                        nullptr, 0.f, rel_scale_thresh, cam_trans, pj2d_org, removed, workspace, sel, img_sel, d_count_out,
+                        (cudaStream_t)stream_);
 }
 
 int b200romp_gather_rows(const void* src, int row_bytes, const int* sel, const int* d_count, int capacity, void* dst,
