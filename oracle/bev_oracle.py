@@ -46,19 +46,36 @@ def block_3d(sd, p, x):
     return y + x
 
 
-def coarse2fine(sd, feat):
-    """coarse2fine_localization + fv_conditioned_bv_estimation, bev/model.py:188-215."""
-    b = feat.shape[0]
+def fv_maps(sd, feat):
+    """det_head and bv_pre_layers on the backbone features (bev/model.py:188-190) -> (maps_fv [B,4,128,128] = center_fv |
+    cam_offset, img_feats [B,16,128,128])."""
     maps_fv = F.conv2d(head_block(sd, "det_head.0.0.", feat), sd["det_head.1.weight"], sd["det_head.1.bias"])
-    center_fv, cam_off = maps_fv[:, :1], maps_fv[:, 1:4]
     x = feat
     for i in (0, 3, 6):
         w = sd[f"bv_pre_layers.{i}.weight"]
         x = F.relu(_bn(sd, f"bv_pre_layers.{i + 1}", F.conv2d(x, w, sd[f"bv_pre_layers.{i}.bias"], 1, w.shape[-1] // 2)))
-    summon = torch.cat([center_fv, cam_off, x], 1).reshape(b, -1, 128)                      # :190
+    return maps_fv, x
+
+
+def bv_input(maps_fv, img_feats):
+    """the bird's-eye input [B, 2560, 128] of bv_out_layers: [center_fv | cam_offset | img_feats] with H folded into C
+    (bev/model.py:190)"""
+    return torch.cat([maps_fv, img_feats], 1).reshape(maps_fv.shape[0], -1, 128)
+
+
+def bv_out(sd, summon):
+    """bv_out_layers: 3 x BasicBlock_1D (bev/model.py:191) -> [B, 128, 128] = center_bv | cam_offset_bv"""
     y = summon
     for i in range(3):
         y = block_1d(sd, f"bv_out_layers.{i}.", y)
+    return y
+
+
+def coarse2fine(sd, feat):
+    """coarse2fine_localization + fv_conditioned_bv_estimation, bev/model.py:188-215."""
+    maps_fv, x = fv_maps(sd, feat)
+    center_fv, cam_off = maps_fv[:, :1], maps_fv[:, 1:4]
+    y = bv_out(sd, bv_input(maps_fv, x))
     center_bv, cam_off_bv = y[:, :64], y[:, 64:]
     center_3d = center_fv.repeat(1, 64, 1, 1) * center_bv.unsqueeze(2).repeat(1, 1, 128, 1)  # :195-196
     center_3d = block_3d(sd, "center_map_refiner.0.", center_3d.unsqueeze(1)).squeeze(1)     # :206

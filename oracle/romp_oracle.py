@@ -154,9 +154,9 @@ def hrnet32_forward(sd, frames_nhwc):
     return xs[0]
 
 
-def coord_maps(size=128):
-    """get_coord_maps, model.py:8-37: ch0 varies along W, ch1 along H, value i/(size-1)*2-1."""
-    r = torch.arange(size, dtype=torch.float32) / (size - 1) * 2 - 1
+def coord_maps(size=128, dtype=torch.float32):
+    """get_coord_maps, model.py:8-37: ch0 varies along W, ch1 along H, value i/(size-1)*2-1 (computed in `dtype`)."""
+    r = torch.arange(size, dtype=dtype) / (size - 1) * 2 - 1
     xx = r.view(1, 1, 1, size).expand(1, 1, size, size)
     yy = r.view(1, 1, size, 1).expand(1, 1, size, size)
     return torch.cat([xx, yy], 1).contiguous()
@@ -164,7 +164,8 @@ def coord_maps(size=128):
 
 def romp_head(sd, feat):
     """ROMPv1.forward after the backbone, model.py:470-481 (+ head layout :445-468)."""
-    x = torch.cat([feat, coord_maps(128).to(feat.device).expand(feat.shape[0], -1, -1, -1)], 1)
+    cm = coord_maps(128, torch.promote_types(feat.dtype, torch.float32))     # fp32, or float64 for float64 features
+    x = torch.cat([feat, cm.to(feat.device).expand(feat.shape[0], -1, -1, -1)], 1)
     outs = {}
     for h in (1, 2, 3):
         q = f"final_layers.{h}."
@@ -178,10 +179,10 @@ def romp_head(sd, feat):
 
 
 @torch.no_grad()
-def romp_maps(sd, frames_nhwc):
-    """Seam S1 (`self.model(x)`, main.py:112) followed by the cam-scale pow of main.py:113."""
+def romp_maps(sd, frames_nhwc, dtype=torch.float32):
+    """Seam S1 (`self.model(x)`, main.py:112) followed by the cam-scale pow of main.py:113, in `dtype` (that of sd)."""
     sd = to_torch_sd(sd)
-    center, params = romp_head(sd, hrnet32_forward(sd, _t(frames_nhwc).float()))
+    center, params = romp_head(sd, hrnet32_forward(sd, _t(frames_nhwc).to(dtype)))
     params = params.clone()
     params[:, 0] = torch.pow(1.1, params[:, 0])
     return center, params
@@ -513,10 +514,11 @@ def resnet50_forward(sd, frames_nhwc):
 
 
 @torch.no_grad()
-def romp_resnet50_maps(sd, frames_nhwc):
-    """ROMP head (same layout as ROMPv1, 64+2 input channels) on the ResNet-50 features + cam-scale pow."""
+def romp_resnet50_maps(sd, frames_nhwc, dtype=torch.float32):
+    """ROMP head (same layout as ROMPv1, 64+2 input channels) on the ResNet-50 features + cam-scale pow, in `dtype`
+    (that of sd)."""
     sd = to_torch_sd(sd)
-    center, params = romp_head(sd, resnet50_forward(sd, _t(frames_nhwc).float()))
+    center, params = romp_head(sd, resnet50_forward(sd, _t(frames_nhwc).to(dtype)))
     params = params.clone()
     params[:, 0] = torch.pow(1.1, params[:, 0])
     return center, params

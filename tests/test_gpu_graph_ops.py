@@ -88,27 +88,40 @@ def _nchw(t):
     return t.permute(0, 3, 1, 2)
 
 
+def conv_linear(x, w, b, *, stride=1, up=1, transpose=False):
+    """the convolution of a conv op, before its residual, ReLU and power: x NHWC, w, b float64 tensors, on x's device.
+    w: OIHW, or [O, I, 3] (Conv1d along W, ksize code 13); transpose: ConvTranspose2d(4, 2, 1) with w in PyTorch's
+    [cin, cout, 4, 4] layout (ksize code 42)"""
+    if transpose:
+        return F.conv_transpose2d(_nchw(x), w, b, stride=2, padding=1).permute(0, 2, 3, 1)
+    return conv_ref(x, w, b, stride=stride, up=up, device=x.device, dtype=torch.float64)
+
+
+def normalise_input(x):
+    """input_norm of a conv op: raw 0..255 values -> x / 255 * 2 - 1 (model.py:385)"""
+    return x / 255.0 * 2.0 - 1.0
+
+
+def pow_f32_11(z):
+    """the pow_channel of a conv op: powf(1.1f, z), the model's fp32 cam scale"""
+    return torch.pow(torch.tensor(F32_11, dtype=torch.float64, device=z.device), z)
+
+
 def conv_bound(x, w, b, *, stride=1, relu=False, res=None, up=1, pow_channel=-1, out_dt=BF16, input_norm=0, transpose=False):
     """float64 result v and per-element bound of one conv op; x, res: NHWC float64 (res may have one frame), w, b float64
     tensors.  input_norm: x holds raw 0..255 values; the kernel's normalised fp32 input carries 2^-22 absolute error.
     transpose: ConvTranspose2d(4, 2, 1) with w in PyTorch's [cin, cout, 4, 4] layout; each output sums 2 x 2 taps per
     input channel, so K = 4 cin."""
     if input_norm:
-        x = x / 255.0 * 2.0 - 1.0
+        x = normalise_input(x)
     if transpose:
         K = 4 * w.shape[0]
-
-        def ref(x_, w_, b_):
-            return F.conv_transpose2d(_nchw(x_), w_, b_, stride=2, padding=1).permute(0, 2, 3, 1)
     else:
         K = w.shape[1] * (w.shape[2] * (w.shape[3] if w.ndim == 4 else 1))
-        kw = dict(stride=stride, up=up, device=x.device, dtype=torch.float64)
-
-        def ref(x_, w_, b_):
-            return conv_ref(x_, w_, b_, **kw)
-    z = ref(x, w, b)
+    kw = dict(stride=stride, up=up, transpose=transpose)
+    z = conv_linear(x, w, b, **kw)
     ax = x.abs() + (2.0 ** -22 if input_norm else 0.0)
-    A = ref(ax, w.abs(), None if b is None else b.abs())
+    A = conv_linear(ax, w.abs(), None if b is None else b.abs(), **kw)
     if res is not None:
         z = z + res
         A = A + res.abs()
@@ -119,7 +132,7 @@ def conv_bound(x, w, b, *, stride=1, relu=False, res=None, up=1, pow_channel=-1,
     if pow_channel >= 0:
         zc = z[..., pow_channel]
         bz = gamma(K) * A[..., pow_channel] + 2.0 ** -23 * zc.abs()
-        vc = torch.pow(torch.tensor(F32_11, dtype=torch.float64, device=x.device), zc)
+        vc = pow_f32_11(zc)
         v[..., pow_channel] = vc
         bound[..., pow_channel] = vc * (F32_11 ** bz - 1) + 2.0 ** -21 * vc
     return v, bound
@@ -152,14 +165,20 @@ def block_bound(x, w1, b1, w2, b2):
     return v, bound
 
 
-def sum_bound(base, terms, ups, relu, out_dt):
-    """fuse-layer sum act(base + sum_k nearest_up(term_k)); base, terms NHWC float64 (already sliced)"""
-    v, a = base.clone(), base.abs()
+def sum_terms(base, terms, ups):
+    """base + sum_k nearest_up(term_k, ups[k]); base, terms NHWC (already sliced)"""
+    v = base.clone()
     for t, u in zip(terms, ups):
         if u > 1:
             t = t.repeat_interleave(u, 1).repeat_interleave(u, 2)
         v = v + t
-        a = a + t.abs()
+    return v
+
+
+def sum_bound(base, terms, ups, relu, out_dt):
+    """fuse-layer sum act(base + sum_k nearest_up(term_k)); base, terms NHWC float64 (already sliced)"""
+    v = sum_terms(base, terms, ups)
+    a = sum_terms(base.abs(), [t.abs() for t in terms], ups)
     if relu:
         v = v.clamp_min(0)
     return v, ROUND[out_dt] * v.abs() + 2.0 ** -24 * (len(terms) + 1) * a
