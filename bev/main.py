@@ -1,6 +1,6 @@
 """``bev.main`` of the reference (simple_romp/bev/main.py): BEV, bev_settings and the lazily evaluated module-level
-``default_settings`` (bev/main.py:61)."""
-from romp_b200.bev import BEV, bev_settings  # noqa: F401
+``default_settings`` (bev/main.py:61), and main(), the ``bev`` command."""
+from romp_b200.bev import BEV, bev_settings, main  # noqa: F401
 
 _default = None
 
@@ -12,3 +12,7 @@ def __getattr__(name):
             _default = bev_settings([])
         return _default
     raise AttributeError(name)
+
+
+if __name__ == "__main__":          # python -m bev.main, like the reference's console script bev=bev.main:main
+    main()

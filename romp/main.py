@@ -12,3 +12,7 @@ def __getattr__(name):
             _default = romp_settings([])
         return _default
     raise AttributeError(name)
+
+
+if __name__ == "__main__":          # python -m romp.main, like the reference's console script romp=romp.main:main
+    main()

@@ -916,3 +916,44 @@ class BEV(torch.nn.Module):
                 self.lib.b200romp_bev_tracker_destroy(self.trk)
         except Exception:
             pass
+
+
+DEFAULT_MODEL_ID = 2     # bev/main.py:23; its video-mode prefix names this default, not --model_id (:304)
+
+
+def check_cli(args):
+    """What the ``bev`` command line refuses, before a model is built: display (with the message of ``BEV``) and any
+    mode but image and video (webcam capture is not provided).  The default --render_mesh is ignored: nothing renders,
+    and the saved PNG is the input frame."""
+    if getattr(args, "show", False):
+        raise NotImplementedError("display (--show) is outside the GPU hot path (SURVEY.md section 2)")
+    if args.mode not in ("image", "video"):
+        raise NotImplementedError("webcam capture is outside the hot path; call BEV.forward per frame")
+
+
+def main(input_args=None):
+    """The ``bev`` command (bev/main.py:289-307) on the batched image path (romp_b200/cli.py).  ``--mode image`` saves
+    ``ResultSaver('image', save_path)``'s files with the prefix ``{center_thresh}``; ``--mode video`` saves every frame
+    with the prefix ``_{2}_{center_thresh}``, then ``video_results.npz`` and with ``--save_video`` the mp4."""
+    from . import cli
+    args = bev_settings(sys.argv[1:] if input_args is None else input_args)
+    check_cli(args)
+    bev = BEV(args)
+    if args.mode == "video":
+        cli.run_video(bev, args, prefix=f"_{DEFAULT_MODEL_ID}_{args.center_thresh}")
+        return
+    run_image(bev, args.input, args.save_path, args.center_thresh)
+
+
+def run_image(bev, input_path, save_path, center_thresh, center3d_override=None):
+    """``--mode image``: one image through ``run_frames``, saved by ``ResultSaver('image', save_path)`` with the prefix
+    ``{center_thresh}`` (bev/main.py:291-296)."""
+    from . import cli
+    import cv2
+    saver = cli.ResultSaver("image", save_path)
+    cli.run_frames(bev, [(input_path, cv2.imread(input_path))], saver, f"{center_thresh}", center3d_override)
+    return saver
+
+
+if __name__ == "__main__":
+    main()

@@ -879,12 +879,28 @@ class ROMP(torch.nn.Module):
 default_settings = None   # the reference evaluates romp_settings([]) at import (main.py:62); we do not
 
 
-def main():
-    import cv2
-    args = romp_settings()
-    romp = ROMP(args)
-    if args.mode != "image":
+def check_cli(args):
+    """What the ``romp`` command line refuses, before a model is built: display and rendering (with the messages of
+    ``ROMP``), and any mode but image and video (webcam capture is not provided)."""
+    for flag in ("render_mesh", "show"):
+        if getattr(args, flag, False):
+            raise NotImplementedError(f"--{flag} is outside the GPU hot path (SURVEY.md section 2: out of scope)")
+    if args.mode not in ("image", "video"):
         raise NotImplementedError("video/webcam loops are outside the hot path; call ROMP.forward per frame")
+
+
+def main(input_args=None):
+    """The ``romp`` command (main.py:178-196).  ``--mode image`` writes ``<save_path>/<input stem>.npz`` when somebody
+    is detected; ``--mode video`` writes the reference's per-frame PNG and npz files, ``video_results.npz`` and with
+    ``--save_video`` the mp4 (romp_b200/cli.py)."""
+    import cv2
+    args = romp_settings(sys.argv[1:] if input_args is None else input_args)
+    check_cli(args)
+    romp = ROMP(args)
+    if args.mode == "video":
+        from . import cli
+        cli.run_video(romp, args)
+        return
     outputs = romp(cv2.imread(args.input))
     if outputs is not None:
         os.makedirs(args.save_path, exist_ok=True)
