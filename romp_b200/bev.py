@@ -24,7 +24,7 @@ import torch
 from . import _lib, graph
 from ._lib import BF16, F32, U8
 from .main import MAX_PERSON, SMPLParser, _ptr, img_preprocess
-from .streams import MAX_VIDEO_STREAMS, check_streams, check_video_streams, stream_indices
+from .streams import MAX_VIDEO_STREAMS, StreamFailed, check_streams, check_video_streams, stream_indices
 from .staging import RawStager, after_producers, frame_buffer, frame_offsets, image_tensor, preprocess_bgr_batch, to_caller
 
 conf_dict = {1: [0.25, 20, 2], 2: [0.1, 20, 1.6]}                    # bev/main.py:24-25
@@ -73,6 +73,12 @@ def bev_settings(input_args=sys.argv[1:]):
                    help=f"with -t: track up to N independent videos (one per signal_ID, each with its own tracker, ids and "
                         f"filters), stepped in parallel on the GPU; 0 = one tracker shared by every signal_ID, like the "
                         f"reference (at most {MAX_VIDEO_STREAMS})")
+    p.add_argument("--inputs", type=str, nargs="+", default=None,
+                   help="--mode video on many videos / frame folders in one process (instead of -i): input p writes into "
+                        "<save_path>/<stem of p>/ what -i p -o <save_path>/<stem of p> writes; with -t each input is its "
+                        "own stream")
+    p.add_argument("--open_inputs", type=int, default=8,
+                   help="--inputs: how many inputs are read at once (cli.OPEN_INPUTS); the others open in order")
     args = p.parse_args(input_args)
     if args.model_id != 2:                                            # bev/main.py:59-63
         args.model_path = osp.join(home, model_dict[args.model_id])
@@ -446,9 +452,9 @@ class BEV(torch.nn.Module):
             self.frame_id = int(h[5])
             if status and self.video_streams:
                 failed = sorted({slot["sids"][b] for b in range(B) if int(h[6 + b]) < 0}, key=repr)
-                raise RuntimeError(f"BEV video mode: more than {TRACKER_MAX_TRACKS} live tracks in the stream(s) of signal_ID "
+                raise StreamFailed(f"BEV video mode: more than {TRACKER_MAX_TRACKS} live tracks in the stream(s) of signal_ID "
                                    f"{', '.join(map(repr, failed))}; call reset_temporal(signal_ID) for each (the other "
-                                   "streams of the batch were tracked)")
+                                   "streams of the batch were tracked)", failed)
             if status:
                 raise RuntimeError("BEV video mode: " + (f"more than {TRACKER_MAX_TRACKS} live tracks" if status == 1 else "too many rows")
                                    + "; call reset_temporal() before the next frame")
@@ -929,18 +935,25 @@ def check_cli(args):
         raise NotImplementedError("display (--show) is outside the GPU hot path (SURVEY.md section 2)")
     if args.mode not in ("image", "video"):
         raise NotImplementedError("webcam capture is outside the hot path; call BEV.forward per frame")
+    from .cli import check_inputs
+    check_inputs(args)
 
 
 def main(input_args=None):
     """The ``bev`` command (bev/main.py:289-307) on the batched image path (romp_b200/cli.py).  ``--mode image`` saves
     ``ResultSaver('image', save_path)``'s files with the prefix ``{center_thresh}``; ``--mode video`` saves every frame
-    with the prefix ``_{2}_{center_thresh}``, then ``video_results.npz`` and with ``--save_video`` the mp4."""
+    with the prefix ``_{2}_{center_thresh}``, then ``video_results.npz`` and with ``--save_video`` the mp4, for ``-i``
+    or for each of ``--inputs``."""
     from . import cli
     args = bev_settings(sys.argv[1:] if input_args is None else input_args)
     check_cli(args)
     bev = BEV(args)
     if args.mode == "video":
-        cli.run_video(bev, args, prefix=f"_{DEFAULT_MODEL_ID}_{args.center_thresh}")
+        prefix = f"_{DEFAULT_MODEL_ID}_{args.center_thresh}"
+        if args.inputs is not None:
+            cli.run_inputs_command(bev, args, prefix)
+        else:
+            cli.run_video(bev, args, prefix=prefix)
         return
     run_image(bev, args.input, args.save_path, args.center_thresh)
 

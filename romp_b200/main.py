@@ -71,6 +71,12 @@ def romp_settings(input_args=sys.argv[1:]):
                         help=f"with -t: track up to N independent videos (one per signal_ID, each with its own tracker, ids "
                              f"and filters), stepped in parallel on the GPU by forward_video(_batches) and forward; 0 = the "
                              f"per-instance signal table (at most {MAX_VIDEO_STREAMS})")
+    parser.add_argument("--inputs", type=str, nargs="+", default=None,
+                        help="--mode video on many videos / frame folders in one process (instead of -i): input p writes "
+                             "into <save_path>/<stem of p>/ what -i p -o <save_path>/<stem of p> writes; with -t each "
+                             "input is its own stream")
+    parser.add_argument("--open_inputs", type=int, default=8,
+                        help="--inputs: how many inputs are read at once (cli.OPEN_INPUTS); the others open in order")
     args = parser.parse_args(input_args)
     if not os.path.exists(args.smpl_path):
         alt = args.smpl_path.replace("SMPL_NEUTRAL.pth", "smpl_packed_info.pth")   # main.py:50-52
@@ -887,19 +893,24 @@ def check_cli(args):
             raise NotImplementedError(f"--{flag} is outside the GPU hot path (SURVEY.md section 2: out of scope)")
     if args.mode not in ("image", "video"):
         raise NotImplementedError("video/webcam loops are outside the hot path; call ROMP.forward per frame")
+    from .cli import check_inputs
+    check_inputs(args)
 
 
 def main(input_args=None):
     """The ``romp`` command (main.py:178-196).  ``--mode image`` writes ``<save_path>/<input stem>.npz`` when somebody
     is detected; ``--mode video`` writes the reference's per-frame PNG and npz files, ``video_results.npz`` and with
-    ``--save_video`` the mp4 (romp_b200/cli.py)."""
+    ``--save_video`` the mp4 (romp_b200/cli.py), for ``-i`` or for each of ``--inputs``."""
     import cv2
     args = romp_settings(sys.argv[1:] if input_args is None else input_args)
     check_cli(args)
     romp = ROMP(args)
     if args.mode == "video":
         from . import cli
-        cli.run_video(romp, args)
+        if args.inputs is not None:
+            cli.run_inputs_command(romp, args)
+        else:
+            cli.run_video(romp, args)
         return
     outputs = romp(cv2.imread(args.input))
     if outputs is not None:

@@ -12,6 +12,15 @@ from __future__ import annotations
 MAX_VIDEO_STREAMS = 1024       # B200ROMP_MAX_VIDEO_STREAMS, include/b200romp.h
 
 
+class StreamFailed(RuntimeError):
+    """Streams of a batch could not be tracked (BEV: a full track table); ``signal_IDs`` lists their signal_IDs.  The
+    other streams of the batch were tracked; each failed one does nothing until ``reset_temporal(signal_ID)``."""
+
+    def __init__(self, message, signal_IDs):
+        super().__init__(message)
+        self.signal_IDs = list(signal_IDs)
+
+
 def check_video_streams(settings, temporal):
     """--video_streams of ``settings``, validated: 0 (one tracker per instance) or 1..MAX_VIDEO_STREAMS with -t."""
     n = int(getattr(settings, "video_streams", 0) or 0)
