@@ -24,6 +24,12 @@
 // Warp roles (384 threads): warp 0 = TMA producer (one elected thread), warpgroups 1 and 2 = consumers.  Each consumer owns
 //            a private ring of pipeline stages and takes every other tile of the CTA, so one warpgroup's epilogue overlaps
 //            the other's MMAs.  Launched with programmatic dependent launch (prologue overlaps the previous conv's tail).
+// SWAP (plan kind 31: bf16 3x3 stride 1, 128 -> 128 channels, bf16 NHWC output): the operands trade places.  The resident
+//            weight slab is A (M = the CTA's 64 output channels; the same image and descriptors as B above) and the 16x8
+//            pixel tile is B (N = 128: its 16 8-pixel groups are halo rows SBO apart, so each tap is the shifted descriptor
+//            of the A operand above, now spanning both halves).  One m64n128k16 reads 2 + 4 KB of shared memory where the
+//            two m64n64k16 read 8 KB.  Chunks, taps and k-steps run in the same order, so the fp32 sums are bit-identical
+//            (tools/wgmma_swap_probe.cu); the accumulators come out channel-major and go through wg_epilogue_swap.
 #include <mutex>
 
 #include "conv_tc.cuh"
@@ -78,11 +84,12 @@ struct TcCfg {
 // kmask: bit (tap * 2 + half) = 0 skips the MMAs of that channel half of that tap (all-zero weights of a pixel-pair folded
 // conv, see net.cu fold_pixel_pairs; single-chunk layers only).  GENERIC: outputs that are not NHWC at conv resolution with
 // whole channel tiles (NCHW maps, 1.1**x, upsampling); the other variant has only the NHWC epilogue (see wg_epilogue).
-template <int MODE, int CIN, int NT, int EB, bool GENERIC>
+template <int MODE, int CIN, int NT, int EB, bool GENERIC, bool SWAP = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ S2Maps s2maps, const ConvParams p,
                const uint8_t* __restrict__ wpack, int tiles_x, int tiles_y, int num_tiles, int stages, unsigned kmask) {
   using Cfg = TcCfg<MODE, CIN, NT, EB>;
+  static_assert(!SWAP || (MODE == 3 && NT == 64 && EB == 2 && !GENERIC), "the swapped plan is bf16 3x3 stride 1, NHWC, M = 64");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sB = smem;
@@ -155,7 +162,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += nrings * gridDim.x) {
       const int n = tile / per_frame, rem = tile % per_frame;
       const int y0 = (rem / tiles_x) * 16, x0 = (rem % tiles_x) * 8;
-      float acc[2][NT / 2];
+      float acc[2][NT / 2];   // SWAP: acc[0] .. acc[1] are the 64 registers of one m64n128 accumulator
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -191,8 +198,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
           for (int k = 0; k < Cfg::KSTEPS; ++k) {
             if (Cfg::FOLDABLE && !((kmask >> (tap * 2 + (k * 2) / Cfg::KSTEPS)) & 1u)) continue;
             const uint64_t bdesc = make_smem_desc(b_tap + k * 32, 8 * Cfg::ROWB, Cfg::LAYOUT);
-            wgmma_any<NT, EB>(acc[0], make_smem_desc(a_tap + k * 32, sbo, Cfg::LAYOUT), bdesc, scale_d);
-            wgmma_any<NT, EB>(acc[1], make_smem_desc(a_tap + 8 * sbo + k * 32, sbo, Cfg::LAYOUT), bdesc, scale_d);
+            if constexpr (SWAP) {
+              wgmma_n128_bf16(*reinterpret_cast<float(*)[64]>(&acc[0][0]), bdesc, make_smem_desc(a_tap + k * 32, sbo, Cfg::LAYOUT), scale_d);
+            } else {
+              wgmma_any<NT, EB>(acc[0], make_smem_desc(a_tap + k * 32, sbo, Cfg::LAYOUT), bdesc, scale_d);
+              wgmma_any<NT, EB>(acc[1], make_smem_desc(a_tap + 8 * sbo + k * 32, sbo, Cfg::LAYOUT), bdesc, scale_d);
+            }
             scale_d = 1;
           }
         }
@@ -206,7 +217,116 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
       }
       wgmma_wait<0>();
       if (wlane == 0) mbar_arrive(&empty[prev]);
-      wg_epilogue<NT, GENERIC ? kEpiGeneric : kEpiNhwc>(p, acc, p.bias, n, y0, x0, blockIdx.y * NT, t);
+      if constexpr (SWAP) {
+        if (p.res != nullptr && p.res_dtype == B200ROMP_F32)
+          wg_epilogue_swap<float2>(p, *reinterpret_cast<float(*)[64]>(&acc[0][0]), n, y0, x0, blockIdx.y * NT, t);
+        else
+          wg_epilogue_swap<uint32_t>(p, *reinterpret_cast<float(*)[64]>(&acc[0][0]), n, y0, x0, blockIdx.y * NT, t);
+      } else {
+        wg_epilogue<NT, GENERIC ? kEpiGeneric : kEpiNhwc>(p, acc, p.bias, n, y0, x0, blockIdx.y * NT, t);
+      }
+    }
+  }
+}
+
+// Streamed weights as A (plan kind 34): bf16 3x3 stride 1, 256 input channels, 64-output-channel slabs, bf16 NHWC output.
+// A 64-channel slab of 256 input channels (295 KB) does not fit next to a pipeline, so it streams through the stage ring
+// with the input: stage = one 32-channel K chunk of the slab's 9 taps (36 KB, M = 64 rows of 64 B, the swizzled image of
+// tc_pack_image) + the 18x18 halo of a 16x16 output tile (20 KB).  A work item is (tile, slab); both consumer warpgroups
+// read every stage, warpgroup g taking the 8-column half g of the tile as B: N = 128, 16 8-pixel groups SBO = 18 halo rows
+// apart, each tap a shifted descriptor.  Per k-step a warpgroup reads 2 + 4 KB for 128 pixels x 64 channels, where the
+// N = 32 plan reads 2 x 3 KB for 128 x 32, and a frame's input is loaded 4 times (once per slab) instead of 8.  The slab
+// costs 295 KB of L2 reads per item.  Chunks, taps and k-steps keep the order of conv_tc_kernel, so the fp32 sums are
+// bit-identical.
+constexpr int kStrmCin = 256, kStrmKch = kStrmCin / 32, kStrmRowB = 64, kStrmHalo = 18;
+constexpr int kStrmWBytes = 9 * 64 * kStrmRowB;                                     // one K chunk of one slab
+constexpr int kStrmHaloPayload = kStrmHalo * kStrmHalo * kStrmRowB;
+constexpr int kStrmStageBytes = kStrmWBytes + (kStrmHaloPayload + 1023) / 1024 * 1024;
+constexpr int kStrmStages = 3;
+constexpr int kStrmSmem = kStrmStages * kStrmStageBytes + 1024 /*barriers*/ + 1024 /*align slack*/;
+static_assert(kStrmSmem <= 227 * 1024, "streamed-weight stages do not fit shared memory");
+
+__global__ void __launch_bounds__(kTcThreads, 1)
+conv_tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const ConvParams p, const uint8_t* __restrict__ wpack, int tiles_x,
+                      int tiles_y, int nslabs, int num_items) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStrmStages * kStrmStageBytes);
+  uint64_t* empty = full + kStrmStages;
+  const int warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStrmStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);   // one arrival per consumer warp: both warpgroups read every stage
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_trigger();
+  const int per_frame = tiles_x * tiles_y;
+
+  if (warp == 0) {
+    // ===================== producer: weights chunk + input halo per stage =====================
+    if (elect_one()) {
+      pdl_wait();
+      const uint64_t pol = l2_policy_stream();
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const int tile = item / nslabs, slab = item % nslabs;
+        const int n = tile / per_frame, rem = tile % per_frame;
+        const int y0 = (rem / tiles_x) * 16, x0 = (rem % tiles_x) * 16;
+        for (int c = 0; c < kStrmKch; ++c) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full[stage], kStrmWBytes + kStrmHaloPayload);
+          uint8_t* dst = smem + (size_t)stage * kStrmStageBytes;
+          bulk_copy_g2s(dst, wpack + ((size_t)slab * kStrmKch + c) * kStrmWBytes, kStrmWBytes, &full[stage]);
+          tma_load_4d(dst + kStrmWBytes, &tmap, &full[stage], c * 32, x0 - 1, y0 - 1, n, pol);
+          if (++stage == kStrmStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================== consumers: warpgroup g takes columns 8g .. 8g + 7 of every tile =====================
+    const int g = (warp >> 2) - 1, t = threadIdx.x & 127, wlane = threadIdx.x & 31;
+    pdl_wait();
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+      const int tile = item / nslabs, slab = item % nslabs;
+      const int n = tile / per_frame, rem = tile % per_frame;
+      const int y0 = (rem / tiles_x) * 16, x0 = (rem % tiles_x) * 16;
+      float acc[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+      uint32_t scale_d = 0;
+      int prev = -1;
+      for (int c = 0; c < kStrmKch; ++c) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t w_base = smem_u32(smem + (size_t)stage * kStrmStageBytes), a_base = w_base + kStrmWBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t a_tap = a_base + (uint32_t)(((tap / 3) * kStrmHalo + tap % 3 + 8 * g) * kStrmRowB);
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            wgmma_n128_bf16(acc, make_smem_desc(w_base + tap * 64 * kStrmRowB + k * 32, 8 * kStrmRowB, kSw64),
+                            make_smem_desc(a_tap + k * 32, kStrmHalo * kStrmRowB, kSw64), scale_d);
+            scale_d = 1;
+          }
+        }
+        wgmma_commit();
+        if (prev >= 0) {                      // the previous stage's MMAs have retired: hand it back to the producer
+          wgmma_wait<1>();
+          if (wlane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == kStrmStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (wlane == 0) mbar_arrive(&empty[prev]);
+      if (p.res != nullptr && p.res_dtype == B200ROMP_F32) wg_epilogue_swap<float2>(p, acc, n, y0, x0 + 8 * g, slab * 64, t);
+      else wg_epilogue_swap<uint32_t>(p, acc, n, y0, x0 + 8 * g, slab * 64, t);
     }
   }
 }
@@ -294,8 +414,8 @@ int tc_pack_weights(const float* w_oihw, int cin, int cout, int taps, int nt, vo
 
 std::string TcConvPlan::describe() const {
   char buf[128];
-  snprintf(buf, sizeof(buf), " [tc%s k%d v%d nt%d grid %dx%d smem %d stages %d%s]", eb == 4 ? "-tf32" : "", kind / 10, kind % 10, nt, grid_x,
-           grid_y, smem_bytes, stages, kmask != 0xFFFFFFFFu ? " pixel-pairs" : "");
+  snprintf(buf, sizeof(buf), " [tc%s k%d v%d nt%d grid %dx%d smem %d stages %d%s]%s", eb == 4 ? "-tf32" : "", kind / 10, kind % 10, nt,
+           grid_x, grid_y, smem_bytes, stages, kmask != 0xFFFFFFFFu ? " pixel-pairs" : "", kind == 31 ? " [tc-swap weights-as-A n128]" : kind == 34 ? " [tc-stream weights-as-A n128 tile 16x16]" : "");
   return buf;
 }
 
@@ -335,6 +455,13 @@ static bool tc_shape_supported(const ConvParams& p, int ksize, int stride) {
 
 static int tc_rowb(int ksize, int stride, int cin, int eb) { return stride == 2 ? s2_row_bytes(cin, eb) : tc_row_bytes(ksize, cin, eb); }
 
+// the streamed-weight plan (kind 34, conv_tc_stream_kernel): bf16 3x3 stride 1, 256 -> 64k channels, 16x16 tiles, bf16 NHWC
+// output at conv resolution
+static bool tc_stream_eligible(const ConvParams& p, int ksize, int stride) {
+  return ksize == 3 && stride == 1 && p.in_dtype == B200ROMP_BF16 && p.cin == kStrmCin && p.cout % 64 == 0 &&
+         p.out_dtype == B200ROMP_BF16 && tc_nhwc_out(p, p.cout) && p.Hout % 16 == 0 && p.Wout % 16 == 0;
+}
+
 // kind, operand bytes, N tile, pipeline stages and shared memory of a plan: the weights stay resident next to >= 2 pipeline
 // stages (>= 1 at stride 2).  false when they do not fit.
 static bool tc_tile(const ConvParams& p, int ksize, int stride, TcConvPlan* plan) {
@@ -342,6 +469,14 @@ static bool tc_tile(const ConvParams& p, int ksize, int stride, TcConvPlan* plan
   const int rowb = tc_rowb(ksize, stride, p.cin, eb), kch = p.cin / (rowb / eb);
   const int budget = 227 * 1024 - 1024 /*align slack*/ - 1024 /*barriers*/;
   auto bbytes = [&](int n) { return ksize * ksize * kch * n * rowb; };
+  if (tc_stream_eligible(p, ksize, stride)) {
+    plan->kind = 34;
+    plan->eb = 2;
+    plan->cin = p.cin; plan->cout = p.cout; plan->nt = 64;
+    plan->stages = kStrmStages;
+    plan->smem_bytes = kStrmSmem;
+    return true;
+  }
   int nt = (p.cout % 64 == 0) ? 64 : 32;
   int stage_bytes, stages;
   if (stride == 2) {
@@ -360,6 +495,10 @@ static bool tc_tile(const ConvParams& p, int ksize, int stride, TcConvPlan* plan
     stages = std::min((budget - bbytes(nt)) / stage_bytes, 8);   // split into two rings (one per consumer warpgroup)
   }
   plan->kind = stride == 2 ? 32 : ksize * 10;
+  // the weights as A (SWAP): bf16 3x3 stride 1, 128 -> 128 channels at N = 64, bf16 NHWC output at conv resolution
+  if (ksize == 3 && stride == 1 && eb == 2 && p.cin == 128 && p.cout == 128 && nt == 64 && p.out_dtype == B200ROMP_BF16 &&
+      tc_nhwc_out(p, p.cout))
+    plan->kind = 31;
   plan->eb = eb;
   plan->cin = p.cin; plan->cout = p.cout; plan->nt = nt;
   plan->stages = stages;
@@ -372,14 +511,19 @@ bool tc_conv_supported(const ConvParams& p, int ksize, int stride) {
   return tc_shape_supported(p, ksize, stride) && tc_tile(p, ksize, stride, &plan);
 }
 
-template <int MODE, int CIN, int NT, int EB>
+template <int MODE, int CIN, int NT, int EB, bool SWAP = false>
 static int launch_inst(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream, bool set_attr_only) {
   if (set_attr_only) {   // plans of one instantiation differ in stages
-    B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    if constexpr (SWAP) {
+      B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    } else {
+      B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<MODE, CIN, NT, EB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    }
     return B200ROMP_OK;
   }
-  auto kern = p.cout % NT == 0 && tc_nhwc_out(p, p.cout) ? conv_tc_kernel<MODE, CIN, NT, EB, false> : conv_tc_kernel<MODE, CIN, NT, EB, true>;
+  auto kern = SWAP ? conv_tc_kernel<MODE, CIN, NT, EB, false, SWAP>
+                   : p.cout % NT == 0 && tc_nhwc_out(p, p.cout) ? conv_tc_kernel<MODE, CIN, NT, EB, false> : conv_tc_kernel<MODE, CIN, NT, EB, true>;
   const int tiles_x = p.Wout / 8, tiles_y = p.Hout / 16;
   const int num_tiles = tiles_x * tiles_y * p.B;
   dim3 grid(std::min(plan.grid_x, num_tiles), plan.grid_y);
@@ -390,6 +534,18 @@ static int launch_inst(const TcConvPlan& plan, const ConvParams& p, cudaStream_t
 
 static int dispatch(const TcConvPlan& plan, const ConvParams& p, cudaStream_t stream, bool attr) {
   const int mode = plan.kind == 32 ? 2 : plan.kind / 10;
+  if (plan.kind == 34) {
+    if (attr) {
+      B2R_CUDA_OK(cudaFuncSetAttribute(conv_tc_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStrmSmem));
+      return B200ROMP_OK;
+    }
+    const int tiles_x = p.Wout / 16, tiles_y = p.Hout / 16, nslabs = p.cout / 64;
+    const int num_items = tiles_x * tiles_y * p.B * nslabs;
+    B2R_CUDA_OK(tc_launch(conv_tc_stream_kernel, dim3(std::min(plan.grid_x, num_items)), kTcThreads, plan.smem_bytes, stream, plan.tmap_in,
+                          p, reinterpret_cast<const uint8_t*>(plan.d_wpack), tiles_x, tiles_y, nslabs, num_items));
+    return B200ROMP_OK;
+  }
+  if (plan.kind == 31 && plan.cin == 128 && plan.nt == 64 && plan.eb == 2) return launch_inst<3, 128, 64, 2, true>(plan, p, stream, attr);
 #define B2R_CASE(M, C, N, E) \
   if (mode == M && plan.cin == C && plan.nt == N && plan.eb == E) return launch_inst<M, C, N, E>(plan, p, stream, attr);
   // bf16
@@ -413,6 +569,23 @@ int tc_conv_prepare(const ConvParams& p, int ksize, int stride, const float* w_o
   if (!tc_tile(p, ksize, stride, plan)) {
     set_error("conv_tc: k%d s%d cin%d does not fit shared memory", ksize, stride, p.cin);
     return B200ROMP_EINVAL;
+  }
+  if (plan->kind == 34) {
+    // the slab image [slab][tap][chunk][64 x 64 B] reordered to [slab][chunk][tap]: one stage's weights are contiguous
+    const std::vector<uint8_t> img = tc_pack_image(w_oihw, p.cin, p.cout, 9, 64, kStrmRowB, 2);
+    std::vector<uint8_t> strm(img.size());
+    const size_t tile = 64 * kStrmRowB;
+    for (int j = 0; j < p.cout / 64; ++j)
+      for (int tap = 0; tap < 9; ++tap)
+        for (int c = 0; c < kStrmKch; ++c)
+          memcpy(strm.data() + (((size_t)j * kStrmKch + c) * 9 + tap) * tile, img.data() + (((size_t)j * 9 + tap) * kStrmKch + c) * tile, tile);
+    plan->d_wpack = upload(strm.data(), strm.size(), allocs);
+    if (!plan->d_wpack) return B200ROMP_ECUDA;
+    plan->grid_x = sm_count;
+    plan->grid_y = 1;
+    const int rc = tc_encode_nhwc_input(&plan->tmap_in, p, 2, 32, kStrmHalo, kStrmHalo, CU_TENSOR_MAP_SWIZZLE_64B, "conv_tc (streamed)");
+    if (rc) return rc;
+    return dispatch(*plan, p, nullptr, true);
   }
   const int eb = plan->eb, rowb = tc_rowb(ksize, stride, p.cin, eb), cw = rowb / eb;
   plan->grid_y = (p.cout + plan->nt - 1) / plan->nt;

@@ -14,7 +14,9 @@ struct S2Maps {
 };
 
 struct TcConvPlan {
-  int kind = 0;                 // kernel family: 10 = 1x1, 30 = 3x3, 32 = 3x3 stride 2, 33 = u8 stem, 13 = conv1d,
+  int kind = 0;                 // kernel family: 10 = 1x1, 30 = 3x3, 31 = 3x3 with the weights as the wgmma A operand
+                                // (conv_tc.cu SWAP), 34 = 3x3 with streamed weights as A (conv_tc_stream_kernel),
+                                // 32 = 3x3 stride 2, 33 = u8 stem, 13 = conv1d,
                                 // 60 = fused 3x3 BasicBlock (conv_block_tc.cu), 70 = fused Bottleneck
                                 // (conv_bottleneck_tc.cu); 0 = none
   int cin = 0, cout = 0, nt = 0;  // channels, output channels per CTA

@@ -363,6 +363,57 @@ __device__ __forceinline__ void wg_epilogue(const ConvParams& p, float (&acc)[2]
   }
 }
 
+// Epilogue of the swapped 3x3 plan (conv_tc.cu SWAP): one 64-channel x 128-pixel accumulator, channel-major.  Thread (warp
+// w, lane l) holds channels co0 + 16w + l/4 + 8e of pixels 8j + 2 (l % 4) + {0, 1} (registers 4j + 2e + {0, 1}); pixel
+// 8j + i of the tile is (y0 + j, x0 + i) of frame n.  Lanes l and l ^ 4 hold channels c and c ^ 1 of the same pixels and
+// swap one fp32 value per pair, so each lane then holds 2 adjacent channels of one pixel and a warp's store covers 16 B of
+// each of 8 pixels, as in wg_epilogue_nhwc.  Bias, residual and ReLU are applied to the same fp32 values in the same order
+// as wg_epilogue, so the bf16 output is bit-identical.  Output bf16 NHWC at conv resolution; residual bf16 (RT = uint32_t,
+// 2 channels) or fp32 (RT = float2), optionally broadcast from frame 0.  The residuals of JB tile rows are loaded before
+// those rows' stores (see wg_epilogue_nhwc on aliasing); JB keeps them at 32 registers.
+template <typename RT, int JB = sizeof(RT) == 4 ? 16 : 8>
+__device__ __forceinline__ void wg_epilogue_swap(const ConvParams& p, const float (&acc)[64], int n, int y0, int x0, int co0,
+                                                 int wg_thread) {
+  const int w = wg_thread >> 5, l = wg_thread & 31, odd = (l >> 2) & 1;
+  const int c = co0 + 16 * w + (l >> 2);           // this lane's accumulator channel for e = 0 (c + 8 for e = 1)
+  const float bias[2] = {__ldg(p.bias + c), __ldg(p.bias + c + 8)};
+  const int ch = c & ~1;                            // the first of the 2 channels this lane stores
+  const size_t pix = ((size_t)n * p.Hout + y0) * p.Wout + x0 + 2 * (l & 3) + odd;   // the pixel it stores, tile row 0
+  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out) + pix * p.out_C + p.out_c_off + ch;
+  const size_t ostep = (size_t)p.Wout * p.out_C;
+  const uint8_t* rbase = nullptr;
+  size_t rstep = 0;
+  if (p.res != nullptr) {
+    const size_t rpix = p.res_broadcast ? pix - (size_t)n * p.Hout * p.Wout : pix;
+    rbase = reinterpret_cast<const uint8_t*>(p.res) + (rpix * p.res_C + p.res_c_off + ch) * (sizeof(RT) / 2);
+    rstep = (size_t)p.Wout * p.res_C * (sizeof(RT) / 2);
+  }
+#pragma unroll
+  for (int j0 = 0; j0 < 16; j0 += JB) {
+    RT rv[JB][2];
+    if (p.res != nullptr) {
+#pragma unroll
+      for (int jj = 0; jj < JB; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) rv[jj][e] = reinterpret_cast<const RT*>(rbase + (j0 + jj) * rstep)[4 * e];   // channel + 8e
+    }
+#pragma unroll
+    for (int jj = 0; jj < JB; ++jj) {
+      const int j = j0 + jj;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float v0 = acc[4 * j + 2 * e] + bias[e], v1 = acc[4 * j + 2 * e + 1] + bias[e];
+        // even lanes keep pixel 0 and send pixel 1, odd lanes the other way round
+        const float recv = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 4);
+        float a = odd ? recv : v0, b = odd ? v1 : recv;
+        if (p.res != nullptr) { const float2 r = res_pair(rv[jj][e]); a += r.x; b += r.y; }
+        if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+        *reinterpret_cast<__nv_bfloat162*>(out + j * ostep + 8 * e) = __floats2bfloat162_rn(a, b);
+      }
+    }
+  }
+}
+
 // launch with the programmatic-stream-serialization attribute (see pdl_trigger / pdl_wait); B200ROMP_NO_PDL=1 disables it
 template <typename... KArgs, typename... Args>
 static inline cudaError_t tc_launch(void (*kern)(KArgs...), dim3 grid, int threads, int smem_bytes, cudaStream_t stream, Args&&... args) {
