@@ -83,7 +83,11 @@ int b200romp_net_add_tensor(b200romp_net* net, int H, int W, int C, int dtype, i
 /* Constant [H,W,C] tensor without batch dimension, uploaded now (e.g. the coord-conv bias map that
  * replaces `torch.cat((x, coordmaps))`, model.py:473). */
 int b200romp_net_add_const_tensor(b200romp_net* net, int H, int W, int C, int dtype, const void* host_data);
-/* weight: host fp32 [cout][cin][k][k] (PyTorch OIHW), bias: host fp32 [cout] or NULL. Returns op id. */
+/* weight: host fp32 [cout][cin][k][k] (PyTorch OIHW), bias: host fp32 [cout] or NULL. Returns op id.
+ * Aliasing rule (add_conv, add_sum, add_maxpool): a slice an op reads of the tensor it writes is either disjoint from the
+ * output slice or, for an elementwise read (a conv residual without res_broadcast, a sum base or an up-1 term), the
+ * identical slice.  A conv input or maxpool input overlapping the output returns B200ROMP_EINVAL.  A chain of convs that
+ * would write over its own input slice is not fused: its convs run one by one. */
 int b200romp_net_add_conv(b200romp_net* net, const b200romp_conv_desc* desc, const float* weight, const float* bias);
 /* Fuse-layer summation of HighResolutionModule.forward (simple_romp/romp/model.py:226-244, nearest upsampling of the
  * higher-index branches :188-197) as ONE elementwise op instead of a chain of residual adds:

@@ -200,10 +200,11 @@ int launch_conv_simt(const ConvParams& p, int ksize, int stride, cudaStream_t st
     return B200ROMP_OK;
   }
   if (ksize == 13 && stride == 1 && p.up == 1) {
-    // Conv1d(k=3) along W (bev/model.py:19-22): rows are independent, so the batch folds into the row index
+    // Conv1d(k=3) along W (bev/model.py:19-22): rows are independent, so the batch folds into the row index - unless the
+    // residual is broadcast: its one frame is indexed by the row within a frame
     ConvParams q = p;
-    q.B = 1; q.Hin = p.B * p.Hin; q.Hout = p.B * p.Hout;
-    dim3 g(((q.Hout + 7) / 8) * ((q.Wout + 7) / 8), (q.cout + 63) / 64, 1);
+    if (!p.res_broadcast) { q.B = 1; q.Hin = p.B * p.Hin; q.Hout = p.B * p.Hout; }
+    dim3 g(((q.Hout + 7) / 8) * ((q.Wout + 7) / 8), (q.cout + 63) / 64, q.B);
     conv_simt_kernel<1, 3, 1><<<g, 256, 0, stream>>>(q);
     B2R_CUDA_OK(cudaGetLastError());
     return B200ROMP_OK;

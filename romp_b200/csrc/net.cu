@@ -158,6 +158,9 @@ static int fill_params(const b200romp_net* net, const Op& op, int batch, bool al
   return B200ROMP_OK;
 }
 
+// channel slices [a, a + n) and [b, b + m) of one tensor share a channel
+static bool slices_overlap(int a, int n, int b, int m) { return a < b + m && b < a + n; }
+
 static int validate_desc(const std::vector<Tensor>& T, const b200romp_conv_desc& d) {
   const int res_c_off = d.res_c_off;
   auto ok_id = [&](int id) { return id >= 0 && id < (int)T.size(); };
@@ -183,6 +186,14 @@ static int validate_desc(const std::vector<Tensor>& T, const b200romp_conv_desc&
     B2R_REQUIRE(tr.H == to.H && tr.W == to.W && !tr.nchw && tr.dtype != B200ROMP_U8, "conv: residual shape/dtype mismatch");
     B2R_REQUIRE(res_c_off >= 0 && res_c_off + d.cout <= tr.C, "conv: residual channel slice out of range");
   }
+  // Aliasing: other CTAs read the input's halo and all its channels while the output is written, so the input slice must not
+  // overlap the output slice of the same tensor; the residual is read elementwise, so it may also be the output slice itself.
+  B2R_REQUIRE(d.in != d.out || !slices_overlap(d.in_c_off, d.cin, d.out_c_off, d.cout),
+              "conv: input slice [%d, %d) of tensor %d overlaps the output slice [%d, %d)", d.in_c_off, d.in_c_off + d.cin, d.in,
+              d.out_c_off, d.out_c_off + d.cout);
+  B2R_REQUIRE(d.res != d.out || !slices_overlap(res_c_off, d.cout, d.out_c_off, d.cout) || (res_c_off == d.out_c_off && !d.res_broadcast),
+              "conv: residual slice [%d, %d) of tensor %d overlaps the output slice [%d, %d) without being it", res_c_off,
+              res_c_off + d.cout, d.res, d.out_c_off, d.out_c_off + d.cout);
   return B200ROMP_OK;
 }
 
@@ -287,6 +298,7 @@ int b200romp_net_add_sum(b200romp_net* net, const b200romp_sum_desc* desc) {
                     tt.H * u == to.H && tt.W * u == to.W,
                 "add_sum: term %d is %dx%dx%d (slice from channel %d), expected %dx%dx%d", k, tt.H, tt.W, tt.C, co, to.H / u, to.W / u, to.C);
   }
+  // aliasing: a base or term that is the output tensor has its shape, so up 1 and the whole, identical slice (elementwise)
   Op op;
   op.kernel = Kernel::Sum;
   op.sum = *desc;
@@ -303,6 +315,7 @@ int b200romp_net_add_maxpool(b200romp_net* net, int in, int out) {
   const Tensor& ti = net->tensors[in];
   const Tensor& to = net->tensors[out];
   B2R_REQUIRE(!ti.nchw && !to.nchw && ti.dtype == to.dtype && ti.dtype != B200ROMP_U8 && ti.C == to.C, "add_maxpool: NHWC bf16/fp32 tensors of equal C");
+  B2R_REQUIRE(in != out, "add_maxpool: input tensor %d is the output tensor (a window is read while its neighbours are written)", in);
   B2R_REQUIRE(to.H == (ti.H + 2 - 3) / 2 + 1 && to.W == (ti.W + 2 - 3) / 2 + 1, "add_maxpool: output must be %dx%d", (ti.H - 1) / 2 + 1, (ti.W - 1) / 2 + 1);
   Op op;
   op.kernel = Kernel::MaxPool;
@@ -475,8 +488,8 @@ struct ChainPattern {
 // Replaces every run of ops that matches `pat` by one op.  Ops i .. i+n-1 fuse when each is a conv as added, of the
 // pattern's shape, and all run on one lane; each intermediate is fusable (fusable_intermediate) and, unless the pattern
 // shares them, read by nothing else; only the last conv adds a residual, and that is the first conv's input slice; the
-// chain's input and output are internal; and the kernel supports the fused op.  A caller that binds an intermediate as an
-// external tensor keeps the convs.
+// chain's input and output are internal, and the output slice does not overlap the input slice; and the kernel supports the
+// fused op.  A caller that binds an intermediate as an external tensor keeps the convs.
 static void fuse_chains(b200romp_net* net, const ChainPattern& pat) {
   std::vector<int> reads, writes;
   count_accesses(net, &reads, &writes);
@@ -496,8 +509,10 @@ static void fuse_chains(b200romp_net* net, const ChainPattern& pat) {
     if (ok) {
       const b200romp_conv_desc& first = c[0].d;
       const b200romp_conv_desc& last = c[n - 1].d;
+      // in place (output slice over the input slice): the fused kernel stages input halos that neighbouring tiles overwrite
       ok = last.res == first.in && last.res_c_off == first.in_c_off && !last.res_broadcast &&
-           !net->tensors[first.in].external && !net->tensors[last.out].external;
+           !net->tensors[first.in].external && !net->tensors[last.out].external &&
+           !(last.out == first.in && slices_overlap(first.in_c_off, first.cin, last.out_c_off, last.cout));
     }
     if (ok) {
       Op f;

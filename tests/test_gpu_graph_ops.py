@@ -479,8 +479,8 @@ def check_op(op, read, batch, frames=None, mutate=None):
         Cc = d1.cin
         w1 = torch.from_numpy(w1.reshape(Cc, Cc, 3, 3)).cuda().double()
         w2 = torch.from_numpy(w2.reshape(Cc, Cc, 3, 3)).cuda().double()
-        b1 = torch.from_numpy(b1).cuda().double()
-        b2 = torch.from_numpy(b2).cuda().double()
+        b1, b2 = (torch.zeros(Cc, dtype=torch.float64, device="cuda") if b is None else torch.from_numpy(b).cuda().double()
+                  for b in (b1, b2))
         x_all = read(d1.in_)[..., d1.in_c_off:d1.in_c_off + Cc]
         if mutate:
             mutate("block", [w1, b1, w2, b2], x_all.double().abs().mean((0, 1, 2)))

@@ -74,6 +74,7 @@ from oracle import bev_oracle as B
 from oracle import romp_oracle as R
 from romp_b200 import _lib, graph, synth
 from romp_b200._lib import U8
+from tests.net_graphs import aliasing_violations
 from tests.test_gpu_graph_ops import (Recorder, conv_linear, excess, maxpool_ref, normalise_input, pow_f32_11, record,
                                       sum_terms)
 
@@ -687,3 +688,16 @@ def test_fake_record_matches_library(monkeypatch, romp_sd, resnet50_sd, bev_sd, 
     for nb in built if kind == "bev" else built[:1]:
         if isinstance(nb, graph.NetBuilder):
             nb.lib.b200romp_net_destroy(nb.net)
+
+
+@pytest.mark.parametrize("kind,precision,switch,env", MATRIX, ids=[f"{k}-{p}-{s}" for k, p, s, _ in MATRIX])
+def test_builder_graphs_keep_aliasing_rule(monkeypatch, romp_sd, resnet50_sd, bev_sd, kind, precision, switch, env):
+    """no graph the builder emits has an op whose read slice of its output tensor overlaps the output slice without
+    being it (include/b200romp.h): the check add_conv / add_maxpool make and the no-fusion rule for in-place chains
+    leave every shipped plan as it was"""
+    sd = dict(romp=romp_sd, resnet50=resnet50_sd, bev=bev_sd)[kind]
+    _, recs = fake_record(monkeypatch, builder(kind, sd, precision), env)
+    for r in recs:
+        assert not aliasing_violations(r), f"{kind} {precision} {switch}: {aliasing_violations(r)}"
+        chains = [d for k, _, a in r["calls"] if k == "conv" for d in [a[0]] if d.res >= 0 and d.res == d.out]
+        assert not chains, f"{kind} {precision} {switch}: in-place residual convs {[(d.in_, d.out) for d in chains]}"
