@@ -335,6 +335,41 @@ int b200romp_preprocess_bgr_batch(const unsigned char* const* imgs_bgr, const in
                                   int n, int out_size, unsigned char* out_rgb_device, float* pad_table, b200romp_stream stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The JPEG round trip of video frames the command lines extract (romp/utils.py:145-151 video2frame writes each frame
+ * with cv2.imwrite('.jpg') and the reference reads it back with cv2.imread): libjpeg-turbo's baseline compressor and
+ * decompressor as OpenCV runs them by default (4:2:0, ISLOW DCT, no restart markers, fancy upsampling), restated in
+ * integer arithmetic so that the bytes and pixels are OpenCV's.  Frame geometry: MCUs of 16 x 16 pixels,
+ * mcus = ceil(w/16) * ceil(h/16), blocks = 6 * mcus in MCU raster order (Y0 Y1 Y2 Y3 Cb Cr).  All buffers belong to the
+ * caller; both calls launch on `stream` and do not synchronize.
+ *   coefs (per frame, DEVICE): int16 [blocks][64], quantized, zig-zag order
+ *   entropy-coded segment (per frame, DEVICE): at most 2 * raw_cap bytes, raw_cap = 4 * ceil((BLOCK_BITS * blocks + 7) / 32),
+ *     BLOCK_BITS = the longest block: an 11-bit DC size code + 11 bits and 63 AC codes of 16 + 10 bits
+ *   encode work (DEVICE, one buffer): sum over frames of 16 + 16 * ceil(blocks / 4) + raw_cap + 4 * ceil(raw_cap / 64)
+ *     bytes, frames in order
+ *   decode work (DEVICE, one buffer): sum over frames of 384 * mcus bytes, frames in order
+ * Tables are HOST arrays: qtables [2][64] (luma, chroma; natural order, 1..255); huff_counts [4][16] and huff_symbols
+ * [4][256] (DC0, AC0, DC1, AC1 as a DHT marker lists them: codes per length 1..16, then the symbols).
+ * ------------------------------------------------------------------------------------------------ */
+#define B200ROMP_JPEG_BLOCK_BITS 1665
+/* jcapistd.c jpeg_write_scanlines through jchuff.c finish_pass, per frame: frame i is the DEVICE pointer imgs_bgr[i]
+ * (h[i] x w[i] BGR pixels, row stride row_stride_bytes[i]; all four are HOST arrays).  jccolor.c rgb_ycc_convert,
+ * jcprepct.c / jcsample.c edge replication and h2v2_downsample, jfdctint.c jpeg_fdct_islow, jcdctmgr.c quantize,
+ * jccoefct.c compress_data's dummy blocks -> coefs[i]; jchuff.c encode_one_block per block (bit lengths, a prefix sum,
+ * then packing in parallel), the 1-bit padding and the 0xFF 0x00 stuffing -> out[i] (the bytes between the SOS header
+ * and EOI), its length into out_bytes[i] (DEVICE int [n]). */
+int b200romp_jpeg_encode_batch(const unsigned char* const* imgs_bgr, const int* h, const int* w, const int* row_stride_bytes,
+                               int n, const unsigned char* qtables, const unsigned char* huff_counts,
+                               const unsigned char* huff_symbols, short* const* coefs, unsigned char* const* out,
+                               int* out_bytes, void* work, b200romp_stream stream);
+/* jdapistd.c jpeg_read_scanlines from the coefficients on: dequantization and jidctint.c jpeg_idct_islow with jdmaster.c's
+ * range-limit table, jdsample.c h2v2_fancy_upsample (h2v2_upsample when ceil(w/2) <= 2) with jdmainct.c's edge rows, and
+ * jdcolor.c ycc_rgb_convert to BGR: coefs[i] (as b200romp_jpeg_encode_batch writes them) -> out_bgr[i] (DEVICE,
+ * h[i] x w[i] x 3, packed rows), the frame cv2.imdecode gives for the encoded bytes.  coefs / out_bgr / h / w are HOST
+ * arrays. */
+int b200romp_jpeg_decode_coefs_batch(const short* const* coefs, const int* h, const int* w, int n, const unsigned char* qtables,
+                                     unsigned char* const* out_bgr, void* work, b200romp_stream stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Row f4: the temporal stage of ROMP.forward with --temporal_optimize (main.py:117-157): One-Euro smoothing of
  * (smpl_thetas, smpl_betas, cam) per tracked person, between seams S2 and S3.  Restates LowPassFilter / OneEuroFilter /
  * create_OneEuroFilter / smooth_results / smooth_global_rot_matrix (utils.py:188-192,203-270) in fp32 on the device; the

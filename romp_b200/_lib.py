@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "lib", "libb200romp.so")
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "pnp.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "romp_track.cu", "resnet_ops.cu"]
+SOURCES = ["net.cu", "conv_simt.cu", "conv_tc.cu", "conv_block_tc.cu", "conv_bottleneck_tc.cu", "conv_stem_tc.cu", "conv1d_tc.cu", "parse.cu", "smpl.cu", "smpl_blend_tc.cu", "project.cu", "pnp.cu", "bev.cu", "pack.cu", "preproc.cu", "temporal.cu", "track.cu", "romp_track.cu", "resnet_ops.cu", "jpeg.cu"]
 
 F32, BF16, U8 = 0, 1, 2
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_WGMMA, ENGINE_TF32 = 0, 1, 2, 3
@@ -180,6 +180,8 @@ def load():
     _sig(lib.b200romp_romp_tracker_reset_stream, i32, vp, i32, vp)
     _sig(lib.b200romp_preprocess_bgr, i32, vp, i32, i32, i32, i32, vp, fp, vp)
     _sig(lib.b200romp_preprocess_bgr_batch, i32, C.POINTER(vp), ip, ip, ip, i32, i32, vp, vp, vp)
+    _sig(lib.b200romp_jpeg_encode_batch, i32, C.POINTER(vp), ip, ip, ip, i32, vp, vp, vp, C.POINTER(vp), C.POINTER(vp), vp, vp, vp)
+    _sig(lib.b200romp_jpeg_decode_coefs_batch, i32, C.POINTER(vp), ip, ip, i32, vp, C.POINTER(vp), vp, vp)
     _sig(lib.b200romp_pack_rows, i32, C.POINTER(vp), ip, i32, vp, i32, i32, i32, i32, vp, i32, vp)
     if lib.b200romp_version() != 200:
         raise RuntimeError("libb200romp.so version mismatch - rebuild")
@@ -209,6 +211,7 @@ EXPORTS = [
     "b200romp_bev_post_frames", "b200romp_bev_crop_post", "b200romp_bev_long_merge_workspace_bytes", "b200romp_bev_long_merge",
     "b200romp_bev_crop_post_images", "b200romp_bev_long_merge_images_workspace_bytes", "b200romp_bev_long_merge_images",
     "b200romp_gather_rows", "b200romp_pack_rows", "b200romp_preprocess_bgr", "b200romp_preprocess_bgr_batch",
+    "b200romp_jpeg_encode_batch", "b200romp_jpeg_decode_coefs_batch",
     "b200romp_tracks_create", "b200romp_tracks_destroy",
     "b200romp_tracks_reset", "b200romp_one_euro_smooth",
     "b200romp_bev_tracker_create", "b200romp_bev_tracker_destroy", "b200romp_bev_tracker_reset", "b200romp_bev_track_step",

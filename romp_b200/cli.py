@@ -87,6 +87,89 @@ def frame_source(input_path, save_path, decode=True):
     return ((p, cv2.imread(p) if decode else None) for p in paths), video_save_path
 
 
+def frame_codec(model):
+    """The GPU JPEG codec (jpeg.FrameCodec) of ``model``'s device, built once per device, or None: for anything but a
+    ROMP or BEV instance on a CUDA device, and when the codec's probe found that the installed OpenCV codes JPEG
+    differently (the reason is printed once)."""
+    from .bev import BEV
+    from .main import ROMP
+    if not isinstance(model, (ROMP, BEV)) or getattr(model.tdevice, "type", None) != "cuda":
+        return None
+    from .jpeg import FrameCodec
+    key = model.tdevice.index
+    with _CODECS_LOCK:
+        if key not in _CODECS:
+            codec = FrameCodec(model.tdevice)
+            if not codec.usable:
+                print(f"Extracting video frames on the CPU: {codec.reason}")
+            _CODECS[key] = codec if codec.usable else None
+        return _CODECS[key]
+
+
+_CODECS, _CODECS_LOCK = {}, threading.Lock()
+
+
+def _extract_gpu(codec, video_path, frame_dir, size):
+    """``_extract`` with the JPEG round trip on the GPU: the frames are read with VideoCapture, and each list of ``size``
+    goes through ``codec`` at once, which writes the same ``.jpg`` bytes and gives the same decoded frames.  Yields
+    (path, decoded device frame, its host copy, event after which the device frame is complete)."""
+    cap = cv2.VideoCapture(video_path)
+    try:
+        pending = []
+
+        def flush():
+            out, event = codec.run([f for _, f in pending])
+            for (path, _), (data, dev, host) in zip(pending, out):
+                with open(path, "wb") as f:
+                    f.write(data)
+                yield path, dev, host, event
+            pending.clear()
+
+        for frame_id in range(int(cap.get(cv2.CAP_PROP_FRAME_COUNT))):
+            ok, frame = cap.read()
+            if not ok:
+                continue
+            pending.append((osp.join(frame_dir, "{:08d}.jpg".format(frame_id)), frame))
+            if len(pending) == size:
+                yield from flush()
+        if pending:
+            yield from flush()
+    finally:
+        cap.release()
+
+
+def model_frames(model, input_path, save_path):
+    """``frame_source(input_path, save_path)`` for ``model``: a video file whose model has a usable GPU codec
+    (``frame_codec``) has its frames extracted through it in lists of ``model.max_batch``, writing the same files and
+    giving the same frames; items are then (path, device frame, host frame, event).  Everything else is
+    ``frame_source``'s (path, image)."""
+    codec = frame_codec(model) if osp.isfile(input_path) else None
+    if codec is None:
+        return frame_source(input_path, save_path)
+    save_dir, video_save_path = output_paths(input_path, save_path)
+    frame_dir = osp.join(save_dir, osp.splitext(osp.basename(input_path))[0] + "_frames")
+    print(f"Extracting the frames of input {input_path} to {frame_dir}")
+    os.makedirs(frame_dir, exist_ok=True)
+    return _extract_gpu(codec, input_path, frame_dir, model.max_batch), video_save_path
+
+
+def model_images(items):
+    """The images the model gets for a list of frame items: a codec frame's device tensor, with the caller's current
+    stream ordered after the codec's work (one event wait per list, no host sync), or the host image."""
+    waited = set()
+    for it in items:
+        if len(it) == 4 and id(it[3]) not in waited:
+            import torch
+            torch.cuda.current_stream(it[1].device).wait_event(it[3])
+            waited.add(id(it[3]))
+    return [it[1] for it in items]
+
+
+def saved_image(item):
+    """The host image a frame item's PNG is written from."""
+    return item[2] if len(item) == 4 else item[1]
+
+
 def collect_frame_path(input_path, save_path):
     """collect_frame_path (romp/utils.py:153-182): extract a video's frames (or list a folder's) and return (frame paths,
     path of the ``--save_video`` file)."""
@@ -264,7 +347,7 @@ def save_video_results(frame_save_paths):
 
 
 def run_frames(model, frames, saver, prefix=None, center_override=None):
-    """Run ``frames`` (an iterable of (frame path, BGR image)) through ``model`` (a ROMP or BEV instance) in lists of
+    """Run ``frames`` (an iterable of (frame path, BGR image), or ``model_frames``' items) through ``model`` (a ROMP or BEV instance) in lists of
     ``model.max_batch`` and save every frame's result in order through ``saver``.
 
     ROMP with -t uses ``forward_video_batches`` (every frame on signal_ID 0), otherwise ``forward_image_batches``; BEV
@@ -278,22 +361,22 @@ def run_frames(model, frames, saver, prefix=None, center_override=None):
     def images():
         for chunk in read_ahead(iter(frames), model.max_batch):
             in_flight.append(chunk)
-            yield [image for _, image in chunk]
+            yield model_images(chunk)
 
     if isinstance(model, ROMP) and model.temporal is not None:
         results = model.forward_video_batches(images(), None, True, center_override)
     else:
         results = model.forward_image_batches(images(), True, center_override)
     for res in results:
-        for (path, image), out in zip(in_flight.popleft(), res):
-            saver(out, path, prefix, image=image)
+        for item, out in zip(in_flight.popleft(), res):
+            saver(out, item[0], prefix, image=saved_image(item))
     saver.close()
 
 
 def run_video(model, args, prefix=None, center_override=None):
     """``--mode video`` (romp/main.py:187-196, bev/main.py:298-307): frames of ``args.input`` through ``run_frames``
     into ``args.save_path``, then ``video_results.npz`` and, with ``--save_video``, the mp4.  Returns the saver."""
-    frames, video_save_path = frame_source(args.input, args.save_path)
+    frames, video_save_path = model_frames(model, args.input, args.save_path)
     saver = ResultSaver("video", args.save_path, writers=WRITERS)
     run_frames(model, frames, saver, prefix, center_override)
     if saver.frame_save_paths:
@@ -501,7 +584,7 @@ def run_inputs(model, inputs, save_path, args, prefix=None, center_override=None
         inp.sent = inp.back = 0
         inp.ended, inp.error, inp.write_failed = False, None, False
         inp.saver = ResultSaver("video", inp.save_dir, pool=pool)
-        inp.reader = _Reader(lambda: frame_source(inp.path, inp.save_dir)[0], model.max_batch, wake)
+        inp.reader = _Reader(lambda: model_frames(model, inp.path, inp.save_dir)[0], model.max_batch, wake)
         live.append(inp)
 
     def stop(inp):
@@ -560,14 +643,14 @@ def run_inputs(model, inputs, save_path, args, prefix=None, center_override=None
                     stop(inp)
             if taken:
                 batch = []
-                for k, (path, image) in taken:
-                    batch.append((live[k], live[k].sent, path, image))
+                for k, item in taken:
+                    batch.append((live[k], live[k].sent, item[0], item))
                     live[k].sent += 1
                 in_flight.append(batch)
                 sids.append([inp.index for inp, _, _, _ in batch])
                 if co is not None:
                     put_override(batch)
-                yield [image for _, _, _, image in batch]
+                yield model_images([item for _, _, _, item in batch])
             elif not live and not waiting:
                 return
             elif not any(x.ended for x in live):
@@ -578,11 +661,11 @@ def run_inputs(model, inputs, save_path, args, prefix=None, center_override=None
             yield sids.popleft()
 
     def save(batch, res):
-        for (inp, _, path, image), out in zip(batch, res):
+        for (inp, _, path, item), out in zip(batch, res):
             inp.back += 1
             if not inp.write_failed:
                 try:
-                    inp.saver(out, path, prefix, image=image)
+                    inp.saver(out, path, prefix, image=saved_image(item))
                 except Exception as e:
                     inp.write_failed = True
                     fail(inp, e)
